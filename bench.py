@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- Viterbi GCUPS (query_L x sum(target_L) / s) of the B200 hot path.
+"""bench.py -- Viterbi GCUPS (query_L x sum(target_L) / s) of the H100 hot path.
 
 Headline workload (`value`, BASELINE.json configs[1], the one the metric is quoted on at one GPU): a synthetic query
 profile L=400 against 100,000 synthetic profile HMMs per GPU (lengths lognormal, median 200, clipped [30,2000]),
@@ -11,18 +11,19 @@ ncclAllGather per step INSIDE the library (hhg_plan_topk; no torch.topk / torch.
     python bench.py --gpus N --steps K --warmup W            (driver; torchrun for N > 1)
     python bench.py --impl reference ...                      (the reference's AVX2 Viterbi on the host cores)
     python bench.py --no-extras                               (skip the configs[2..4] sections)
+    python bench.py --dump-outputs DIR                        (write the timed path's last-step results as DIR/*.npy)
 
 value  : whole-job GCUPS, database resident in HBM, device-timed (CUDA events, max over ranks)
 e2e    : the same through the host-buffer C-ABI calls (hhg_query_set + hhg_viterbi_search + hhg_plan_topk): per step
          the query profile and the target-id list go H2D from pinned memory, hits and paths come back D2H.
 roofline : algorithmic bytes (112 B per target column + 1 B per DP cell + 40 B per hit) / forward-kernel time against
-         the measured HBM peak (frac = frac_hbm), and the issue-slot fraction (frac_issue) that actually binds.
+         the HBM peak (frac = frac_hbm); the exact-fp32 recurrence is bound by instruction issue, not by HBM.
 verified : number of hits of the TIMED run compared with the C oracle (score bits, end points, path) in here.
 cpu_baseline / --impl reference : the reference's own Viterbi::Align + Backtrace (oracle/_ref, AVX2) on a bounded
          sample drawn from the SAME rank-0 shard, threads = min(affinity, cgroup quota), OMP_PROC_BIND=close.
 configs : the other north_star configurations, each with per-stage ms:
-         N = 1: configs[2] (1M HMMs, prefilter + Viterbi, one GPU) and configs[4] on one GPU (Lq=1500, full scan);
-         N > 1: configs[3] (1M sharded N ways, prefilter -> Viterbi on survivors -> NCCL top-K) and configs[4].
+         N = 1: configs[2] (--total-targets HMMs, default 300k, prefilter + Viterbi, one GPU) and configs[4] on one GPU (Lq=1500, full scan);
+         N > 1: configs[3] (--total-targets sharded N ways, prefilter -> Viterbi on survivors -> NCCL top-K) and configs[4].
 """
 from __future__ import annotations
 
@@ -41,8 +42,7 @@ sys.path.insert(0, ROOT)
 
 TOPK = 500          # realign_max of the reference (src/hhdecl.cpp): records exchanged per rank
 BASE_SEED = 1000
-# instructions per 32-cell row visit of k_viterbi<16,local> (ncu smsp__inst_executed / row visits, profiles/r2_*)
-WARP_INSTR_PER_ROW_VISIT = 105.7
+DUMP_PATH_SAMPLE = 256   # --dump-outputs: targets whose alignment paths are written (fixed seed)
 
 
 def parse_args():
@@ -52,14 +52,37 @@ def parse_args():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--targets", type=int, default=100000, help="targets per GPU of the headline workload")
-    ap.add_argument("--total-targets", type=int, default=1000000, help="database size of configs[2..4]")
+    # 300k HMMs: configs[4] (Viterbi over the whole database at Lq=1500) holds the shard, its operand stream, boundary
+    # slots, paths and a 0.45-of-HBM backtrace wave at once, which fits one 80 GB H100 next to the e2e section's plan
+    ap.add_argument("--total-targets", type=int, default=300000, help="database size of configs[2..4]")
     ap.add_argument("--lq", type=int, default=400)
     ap.add_argument("--cpu-sample", type=int, default=4000, help="targets in the cpu_baseline sample")
     ap.add_argument("--ref-sample", type=int, default=8000, help="targets per step of --impl reference")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the configs[2..4] sections")
     ap.add_argument("--no-prefilter", action="store_true", help="(kept for old command lines; same as --no-extras)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step computed as DIR/<name>.npy")
     return ap.parse_args()
+
+
+def dump_outputs(outdir, prefix, hits, paths, merged):
+    """The last timed step's results as float32/float64 .npy files: every hit record field of the shard (path_off, a
+    layout offset, excepted), the alignment paths of a fixed seeded sample of targets, and the merged top-K list."""
+    os.makedirs(outdir, exist_ok=True)
+    out = {f"hits_{f}": hits[f].astype(np.float32) for f in HIT_FIELDS}
+    pick = np.sort(np.random.default_rng(BASE_SEED).choice(len(hits), min(DUMP_PATH_SAMPLE, len(hits)), replace=False))
+    out["path_sample_targets"] = pick.astype(np.float32)
+    out["path_sample_states"] = np.concatenate(
+        [paths[int(hits[t]["path_off"]):int(hits[t]["path_off"]) + int(hits[t]["nsteps"])] for t in pick]).astype(np.float32)
+    out["topk_target"] = merged["target"].astype(np.float64)
+    for f in HIT_FIELDS:
+        out[f"topk_{f}"] = merged["hit"][f].astype(np.float32)
+    for name, a in out.items():
+        np.save(os.path.join(outdir, f"{prefix}{name}.npy"), a)
+
+
+HIT_FIELDS = ("score", "i2", "j2", "i1", "j1", "nsteps", "matched_cols", "hit_score", "score_ss")
 
 
 # ----------------------------------------------------------------------------------------------- host facts
@@ -135,21 +158,31 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0}, "fallback"
+        return {"hbm_gbs": 3350.0}, "H100 SXM data sheet (not reached)"
 
 
-def captured_traffic(key):
-    """dram__bytes_read+write per launch of the dominant kernel from the committed ncu capture of this workload."""
+def gpu_info(dev):
+    """Name, SM count and power limit of the measuring GPU: they belong next to every number taken on it."""
+    import torch
+    p = torch.cuda.get_device_properties(dev)
+    info = {"name": p.name, "sms": p.multi_processor_count, "power_limit_w": None}
     try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            t = json.load(f)
-        return t.get(key)
+        import pynvml
+        pynvml.nvmlInit()
+        h = pynvml.nvmlDeviceGetHandleByIndex(ClockSampler(dev.index)._nvml_index())
+        info["power_limit_w"] = pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
     except Exception:
-        return None
+        try:
+            out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i",
+                                  str(ClockSampler(dev.index)._nvml_index())], capture_output=True, text=True, timeout=20)
+            info["power_limit_w"] = float(out.stdout.strip().splitlines()[0])
+        except Exception:
+            pass
+    return info
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md's clocks line).
+    """SM clock and throttle reasons sampled DURING the timed region.
     NVML in a thread (5 ms period) is the sampler; if NVML cannot be loaded, `nvidia-smi -lms 20` is, and start()
     then waits for its first line (a fresh box can take seconds to deliver it -- longer than the timed region)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -374,7 +407,7 @@ def subset_db(base, idx):
 
 
 def extras(args, hh, ctx, comm, rank, world, dev, qprof, base, dist):
-    """configs[2] / configs[3] (1M HMMs, two-stage prefilter -> Viterbi on the survivors -> top-K) and configs[4]
+    """configs[2] / configs[3] (--total-targets HMMs, two-stage prefilter -> Viterbi on the survivors -> top-K) and configs[4]
     (Lq=1500, Viterbi over the whole database), the database = the 100k rank-0 base repeated to --total-targets and
     sharded N ways by shard.balanced_shards.  Returns a dict of per-stage times."""
     import torch
@@ -648,31 +681,21 @@ def main():
     if world == 1 and not np.array_equal(merged["target"], gids[order]):
         raise SystemExit("bench verification FAILED: device top-K differs from the host sort")
     verified += len(own)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, f"rank{rank}_" if world > 1 else "", hits, paths, merged)
 
     # ---- per-kernel roofline figure (forward kernel timed alone with CUDA events on the same stream)
     kt = [plan.run_timed() for _ in range(3)]
     ms_vit = float(np.mean([a for a, b in kt])); ms_bt = float(np.mean([b for a, b in kt]))
     peaks, peak_src = measured_peaks()
     ach = plan.alg_bytes / (ms_vit * 1e-3) / 1e9
-    default_wl = (args.targets == 100000 and args.lq == 400)
-    traffic = captured_traffic("k_viterbi_16_local_100k_lq400") if default_wl else None
-    sm_mhz = clocks.get("sm_mhz") or 1965.0
-    row_visits = cells_rank / 32.0
-    issue_cycles = row_visits * WARP_INSTR_PER_ROW_VISIT / (148 * 4)          # per SMSP at 1 warp-instruction / clock
-    frac_issue = issue_cycles / (ms_vit * 1e-3 * sm_mhz * 1e6)
     roofline = {"bound": "issue", "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                "frac": ach / peaks["hbm_gbs"], "frac_hbm": ach / peaks["hbm_gbs"], "frac_issue": frac_issue,
-                "traffic": traffic["bytes"] if traffic else None,
-                "traffic_source": traffic["source"] if traffic else None,
-                "traffic_over_algorithmic": (traffic["bytes"] / plan.alg_bytes) if traffic else None,
+                "frac": ach / peaks["hbm_gbs"], "frac_hbm": ach / peaks["hbm_gbs"],
                 "peak_source": peak_src, "kernel": "k_viterbi<16,local>", "kernel_ms": ms_vit, "backtrace_ms": ms_bt,
                 "algorithmic_bytes_per_launch": plan.alg_bytes,
                 "kernel_gcups": cells_rank / (ms_vit * 1e-3) / 1e9,
-                "issue_model": f"{WARP_INSTR_PER_ROW_VISIT} warp instructions per 32-cell row visit (ncu) on 592 SMSPs at "
-                               f"{sm_mhz:.0f} MHz (sampled); the ALU and FMA pipes each carry ~73 cycles of that",
-                "note": "exact-fp32 max-plus recurrence: FP32-issue bound, not HBM bound (DESIGN.md 4.1, SURVEY 8d); frac "
-                        "is the algorithmic-bytes fraction of the measured HBM peak as the contract asks, frac_issue is "
-                        "the fraction of the issue-slot ceiling"}
+                "note": "exact-fp32 max-plus recurrence: bound by instruction issue, not by HBM (DESIGN.md 4.1); frac "
+                        "is the algorithmic-bytes fraction of the HBM peak"}
 
     # ---- end to end through the host-buffer C-ABI call, pinned host buffers
     pin = lambda a: torch.from_numpy(a).pin_memory().numpy()  # noqa: E731
@@ -716,10 +739,12 @@ def main():
                         "(loaded once, like the reference's mmap'd ffindex DB)"},
         "gpu_launches": int(launches),
         "verified": int(verified),
+        "gpu": gpu_info(dev),
         "clocks": clocks,
         "roofline": roofline,
         "sum_target_L_this_rank": int(db_h["L"].sum()),
     }
+    plan.close(); db.close()             # the headline shard's HBM goes back before the larger configs load theirs
     if not args.no_extras:
         out["configs"] = extras(args, hh, ctx, comm, rank, world, dev, qprof, db_h if rank == 0 and world == 1 else
                                 headline_shard(args, 0, 1)[1], dist)
@@ -739,7 +764,6 @@ def main():
                                    "sample": "reference arm failed: " + (r.stderr or r.stdout)[-300:]}
     if rank == 0:
         args.emit(out)
-    plan.close(); db.close()
     if comm is not None:
         comm.close()
     ctx.close()

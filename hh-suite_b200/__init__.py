@@ -1,4 +1,4 @@
-"""hh-suite_b200: B200-native Viterbi HMM-HMM alignment + cs219 prefilter behind the HH-suite3 call
+"""hh-suite_b200: GPU-native (H100) Viterbi HMM-HMM alignment + cs219 prefilter behind the HH-suite3 call
 boundary.  The product is the C-ABI library (include/hhg.h, csrc/); this package is its thin host
 mirror in Python (ctypes) plus the synthetic-data generator used by tests and bench.py."""
 from . import build, capi, ffindex, mac, pipeline, prefilter, runner, shard, synth  # noqa: F401

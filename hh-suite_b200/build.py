@@ -1,4 +1,4 @@
-"""Build the product library in-tree: hh-suite_b200/libhhg.so (sm_100a only, no other arch)."""
+"""Build the product library in-tree: hh-suite_b200/libhhg.so (sm_90a only, no other arch)."""
 from __future__ import annotations
 
 import os
@@ -14,7 +14,7 @@ DEPS = sorted(glob.glob(os.path.join(HERE, "csrc", "*.cu*")) + glob.glob(os.path
               glob.glob(os.path.join(os.path.dirname(HERE), "include", "*.h")))
 OUT = os.path.join(HERE, "libhhg.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-fmad=false",            # belt and braces: the kernels use explicit _rn intrinsics anyway
          "-Xcompiler", "-fPIC", "-Xcompiler", "-ffp-contract=off",   # host-side flog2/fpow2 must not be fused either
          "-diag-suppress", "177", "-shared"]

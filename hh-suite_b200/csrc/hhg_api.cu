@@ -1,4 +1,4 @@
-// hh-suite_b200/csrc/hhg_api.cu -- the C-ABI (include/hhg.h) over the sm_100a kernels.
+// hh-suite_b200/csrc/hhg_api.cu -- the C-ABI (include/hhg.h) over the sm_90a kernels.
 // Host side: planning (length-sorted 32-target warp jobs, strip work items, memory waves),
 // device memory, launches.  There is no CPU fallback: without a CUDA device every entry point fails.
 #include "../../include/hhg.h"
@@ -255,10 +255,9 @@ int hhg_ctx_create(int device, void* stream, hhg_ctx** out) {
   CK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  // sm_100a code only loads on compute capability 10.0; the fence-free 256-bit slot hand-off of k_viterbi was
-  // validated on exactly that part (tests/test_kernel_variants_gpu.py stress test)
-  if (prop.major != 10 || prop.minor != 0)
-    return fail(HHG_ENODEV, "device %d is sm_%d%d; this library is built and validated for sm_100a (B200) only", device,
+  // sm_90a code only loads on compute capability 9.0 (H100)
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(HHG_ENODEV, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device,
                 prop.major, prop.minor);
   std::unique_ptr<hhg_ctx> holder(new hhg_ctx());
   hhg_ctx* c = holder.get();
@@ -582,8 +581,7 @@ int msa_chunk_run(hhg_ctx* ctx, MsaChunk& C, const hhg_msa_params& mp, const flo
   MSA_CK(cudaMemsetAsync(C.tr.p, 0, nc * 7 * 4, ctx->stream));
   const float* rcp = msa_rcp_table(ctx);
   if (!rcp) return fail(HHG_ECUDA, "reciprocal table upload failed");
-  int sms = 148;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
+  const int sms = ctx->sm_count;
   // k_msa_mstate is latency bound inside a block (ordered sums, barriers): 12 blocks of 128 threads per SM = its register /
   // shared-memory residency (40 registers, 16 KB), every block pulls (alignment, column) items until the queue is empty
   const int nblk = (int)std::min<long long>((long long)sms * 12, std::max<long long>(items, 1));
@@ -1849,7 +1847,6 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
     P.celloff = pl->celloff ? pl->d_co.p : nullptr;
     P.S33 = ctx->has_S33 ? ctx->S33.p : nullptr;
     P.egq = ctx->par.egq; P.egt = ctx->par.egt; P.shift = ctx->par.shift; P.ssw = ctx->par.ssw;
-    P.one2 = 0x3F8000003F800000ull;
     P.zero = 0u;
 
     const int items = P.n_items;

@@ -786,8 +786,7 @@ k_msa_weights(MsaArrays A, int* __restrict__ ni_all) {
 // residue changes owns the whole run of columns up to the next change: it builds the sub-alignment counts n[j][a],
 // the weights wi[k], Neff of the run, and then the emission frequencies and M->x transitions of every column of the run.
 // Block size: most of a block's time is ordered (single-thread or thread-per-row) work between barriers, so many small
-// blocks beat few large ones: 128 threads, 16 KB of shared memory, 40 registers -> 12 resident blocks per SM (ncu of the
-// 256-thread version: 28 % issue-active, barrier = the top stall).
+// blocks beat few large ones: 128 threads, 16 KB of shared memory, 40 registers -> 12 resident blocks per SM.
 __global__ void __launch_bounds__(MSA_MSTATE_THREADS)
 k_msa_mstate(MsaArrays A, int n_msa, const long long* __restrict__ item_off, long long n_items, int* __restrict__ counter,
              int* __restrict__ cnt_all, float* __restrict__ wc_all, float* __restrict__ wi_all, uint8_t* __restrict__ mem_all,

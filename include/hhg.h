@@ -1,4 +1,4 @@
-/* include/hhg.h -- C-ABI of the B200-native HH-suite hot path (Viterbi HMM-HMM alignment +
+/* include/hhg.h -- C-ABI of the GPU-native (H100, sm_90a) HH-suite hot path (Viterbi HMM-HMM alignment +
  * cs219 ungapped prefilter).  Plain pointers and sizes only; no torch / C++ types.
  *
  * This is the boundary a reference maintainer binds to.  The reference (soedinglab/hh-suite) has no
@@ -45,7 +45,7 @@ extern "C" {
 #define HHG_EINVAL (-1)   /* bad argument */
 #define HHG_ECUDA (-2)    /* CUDA runtime error (message in hhg_last_error) */
 #define HHG_ENOMEM (-3)   /* device or host allocation failed */
-#define HHG_ENODEV (-4)   /* no usable sm_100 device: there is NO CPU fallback */
+#define HHG_ENODEV (-4)   /* no usable sm_90 device: there is NO CPU fallback */
 
 typedef struct hhg_ctx hhg_ctx;   /* one GPU + one stream + scratch */
 typedef struct hhg_db hhg_db;     /* a device-resident shard of prepared target profiles */

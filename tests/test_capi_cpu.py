@@ -1,4 +1,4 @@
-"""CPU tests of the C-ABI library: it builds for sm_100a, loads, exports every symbol include/hhg.h
+"""CPU tests of the C-ABI library: it builds for sm_90a, loads, exports every symbol include/hhg.h
 declares, and refuses to run without a GPU (no CPU fallback)."""
 import os
 import re
@@ -18,11 +18,11 @@ def test_exports_match_header(hhg):
     assert set(hhg.capi.SYMBOLS) <= declared
 
 
-def test_sass_is_sm100a_only():
+def test_sass_is_sm90a_only():
     import subprocess
     so = os.path.join(ROOT, "hh-suite_b200", "libhhg.so")
     out = subprocess.run(["cuobjdump", "-lelf", so], capture_output=True, text=True).stdout
-    assert "sm_100a" in out and "sm_90" not in out and "sm_80" not in out
+    assert "sm_90a" in out and "sm_100" not in out and "sm_80" not in out
 
 
 @pytest.mark.skipif(os.path.exists("/dev/nvidiactl"), reason="GPU present")

@@ -4,7 +4,7 @@ host tokeniser against the oracle's."""
 import numpy as np
 import pytest
 
-from tests.util import bits, golden
+from tests.util import bits, golden, ref_data, ref_data_file
 
 
 def _params(G):
@@ -39,7 +39,7 @@ def test_oracle_fast_log2_table_equals_reference(oracle):
 def test_oracle_prepare_equals_compiled_reference(oracle, refshim, tmp_path, seed):
     from hhsuite_b200 import synth
     rng = np.random.default_rng(seed)
-    refshim.load_query_hhm(str(_query_path()))
+    refshim.load_query_hhm(ref_data_file("query.hhm", tmp_path))
     R, pp = refshim.R(), refshim.prep_params()
     for k in range(4):
         L = int(rng.integers(1, 500))
@@ -60,20 +60,11 @@ def test_oracle_prepare_equals_compiled_reference(oracle, refshim, tmp_path, see
             assert not out["ss"].any()
 
 
-def _query_path():
-    import os
-    from tests.util import ROOT
-    for p in (os.path.join(ROOT, "oracle", "_ref", "data", "query.hhm"), "/root/reference/data/query.hhm"):
-        if os.path.exists(p):
-            return p
-    pytest.skip("data/query.hhm not available")
-
-
 def test_product_tokeniser_equals_oracle(oracle):
     """hhg_hhm_parse (the host half of hhg_db_create_hhm; no GPU needed) against the oracle's parser."""
     from hhsuite_b200 import capi, synth
     G = golden()
-    texts = [G["hhm_ss60_text"].tobytes(), G["hhm_t150_text"].tobytes(), open(_query_path(), "rb").read()]
+    texts = [G["hhm_ss60_text"].tobytes(), G["hhm_t150_text"].tobytes(), ref_data("query.hhm")]
     texts += [synth.hhm_text(L, 70 + k, f"x{k}", with_ss=ss).encode()
               for k, (L, ss) in enumerate([(1, False), (2, True), (333, False), (800, True)])]
     texts.append(texts[0] + b"\0trailing garbage that an ffindex neighbour would be")

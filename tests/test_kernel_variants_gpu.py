@@ -65,7 +65,7 @@ def test_long_query_many_strips(hhg, oracle, cfg):
 
 
 def test_handoff_stress_many_epochs_and_concurrent_contexts(hhg, oracle):
-    """The strip hand-off relies on tagged 32-byte slots (one STG.256 / LDG.256, no fences).  Hammer it: small
+    """The strip hand-off relies on tagged 64-bit words (relaxed loads and stores, no fences).  Hammer it: small
     strips (R=8 -> 50 strips), 300 runs of the same plan (slot memory is reused, only the epoch in the tag
     changes), three contexts on their own streams and host threads at once, as hhblits_omp drives the path
     (src/hhblits_omp.cpp:119-138).  Every run must reproduce the first run's bits; the first run is checked

@@ -10,6 +10,20 @@ def golden():
     return np.load(os.path.join(ROOT, "tests", "golden", "golden_v1.npz"))
 
 
+def ref_data(name):
+    """Bytes of a data file shipped with the reference release (query.hhm, cs219.lib), stored under tests/golden."""
+    with np.load(os.path.join(ROOT, "tests", "golden", "refdata_v1.npz")) as z:
+        return z[name.replace(".", "_")].tobytes()
+
+
+def ref_data_file(name, directory):
+    """ref_data(name) written to directory/name; returns the path as a string."""
+    path = os.path.join(str(directory), name)
+    with open(path, "wb") as f:
+        f.write(ref_data(name))
+    return path
+
+
 def bits(x):
     return np.asarray(x, np.float32).view(np.uint32)
 

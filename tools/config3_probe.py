@@ -1,4 +1,4 @@
-"""BASELINE configs[2] at full size: query L=400 vs N (default 1M) synthetic HMMs on one B200,
+"""BASELINE configs[2] at full size: query L=400 vs N (default 1M) synthetic HMMs on one GPU,
 two-stage cs219 prefilter over the whole shard + Viterbi (with Hit.score, backtrace) on the survivors.
     python tools/config3_probe.py [N] [planted_homologs]
 Prints wall-clock per query (host + device, PCIe included) and its breakdown."""
