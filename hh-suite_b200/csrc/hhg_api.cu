@@ -1629,14 +1629,16 @@ static int plan_build(hhg_ctx* ctx, hhg_plan* pl, const hhg_db* db, int n, const
   auto A = [&](cudaError_t r) { if (e == cudaSuccess) e = r; };
   A(pl->d_job_target.ensure(job_target.size())); A(pl->d_job_Lmax.ensure(pl->njobs));
   A(pl->d_job_bt_off.ensure(pl->njobs)); A(pl->d_job_bnd_off.ensure(pl->njobs)); A(pl->d_job_co_off.ensure(pl->njobs));
-  A(pl->d_job_jc_off.ensure(pl->njobs)); A(pl->d_jcols.ensure((size_t)jc));
+  // one column (224 float4) and one slot column (32 slots) of slack: k_viterbi prefetches column j+1 unconditionally,
+  // so at the last job's last column it reads one column past the operand stream and the slots (never used)
+  A(pl->d_job_jc_off.ensure(pl->njobs)); A(pl->d_jcols.ensure((size_t)jc + 224));
   A(pl->d_job_query.ensure(pl->njobs)); A(pl->d_job_nstrips.ensure(pl->njobs)); A(pl->d_job_Lq.ensure(pl->njobs));
   A(pl->d_job_qrow0.ensure(pl->njobs)); A(pl->d_job_ss_off.ensure(pl->njobs)); A(pl->d_items.ensure(pl->items.size()));
   A(pl->d_req_job.ensure(n)); A(pl->d_req_lane.ensure(n)); A(pl->d_req_Lt.ensure(n)); A(pl->d_req_Lq.ensure(n));
   A(pl->d_path_off.ensure(n));
   A(pl->d_req_target.ensure(n)); A(pl->d_S.ensure((size_t)po));
   A(pl->d_bt.ensure(max_wave_words));
-  { BndSlot* before = pl->d_bnd.p; A(pl->d_bnd.ensure((size_t)bnd));
+  { BndSlot* before = pl->d_bnd.p; A(pl->d_bnd.ensure((size_t)bnd + 32));
     // fresh slots must not carry a bit pattern that looks like a valid tag (epochs start at 1)
     if (e == cudaSuccess && pl->d_bnd.p != before) A(cudaMemsetAsync(pl->d_bnd.p, 0, pl->d_bnd.n * sizeof(BndSlot), ctx->stream)); }
   A(pl->d_strip_score.ensure((size_t)ss * 32));

@@ -243,26 +243,33 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
     const int t = P.job_target[job * 32 + lane];
     const int Lt = P.Lt[t];
     const int Lmax = P.job_Lmax[job];
-    const float4* jc = P.jcols + P.job_jc_off[job] + lane;   // operand k of column j: jc[((j-1)*7+k)*32]
-    uint32_t* btj = P.bt + P.job_bt_off[job] + lane;
+    // per-column pointers advance by constants: the operand stream by 7 x 32 float4, slots and backtrace words by 32.
+    // The plan allocates one column of slack after the last job's stream and slots, so the prefetch of column j+1
+    // needs no clamp (what it reads after the job's last column is never used)
+    const float4* jc = P.jcols + P.job_jc_off[job] + lane;   // operand k of the prefetched column: jc[k*32]
     const size_t bt_row_stride = (size_t)(Lmax + 1) * 32;   // words per 4-row group
-    BndSlot* bnd = P.bnd + P.job_bnd_off[job];                // slots of column j: bnd + j*32
+    uint32_t* btc = P.bt + P.job_bt_off[job] + lane + (size_t)(i0 >> 2) * bt_row_stride + 32;   // column j
+    BndSlot* bndc = P.bnd + P.job_bnd_off[job] + 32;          // the job's 32 slots of column j
     const uint32_t tag_in = P.tag_base + (uint32_t)s;        // written by strip s-1
     const uint32_t tag_out = P.tag_base + (uint32_t)s + 1u;  // what this strip writes
     const bool last_strip = (s == nstrips - 1);
-    const uint32_t* co = nullptr;
-    if (CELLOFF) co = P.celloff + P.job_co_off[job] + (size_t)s * (Lmax + 1) * 32 + lane;
+    const uint32_t* co = nullptr;                            // column j
+    if (CELLOFF) co = P.celloff + P.job_co_off[job] + (size_t)s * (Lmax + 1) * 32 + lane + 32;
 
-    // ---- state of the R rows at the previous column (column 0 initially), :161-173
-    float MM[R], GD[R], IM[R], DG[R], MI[R];
+    // ---- state of the R rows at the previous column (column 0 initially), :161-173.
+    // Every array element is read by its own row before the row overwrites it, so the state updates in place:
+    //   * MI is not kept.  Its two readers are row r+1's c5 at column j+1 (diagonal) and row r+1's mi at column j
+    //     (up), and both add q_m2m(r+1) first; Y[r] = MI(r-1, j-1) + q_m2m(r) is that shared sum.
+    //   * the other diagonal reads (c1..c4 of row r+1) take partial sums that row r forms from its old values
+    //     before it overwrites them (pMM, pGD, pIM, pDG).
+    float MM[R], GD[R], IM[R], DG[R], Y[R];
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       MM[r] = __fmul_rn((float)(-(i0 + 1 + r)), P.egq);
-      GD[r] = IM[r] = DG[r] = MI[r] = HHG_NEG;
+      GD[r] = IM[r] = DG[r] = HHG_NEG;
     }
     // boundary row i0 at column j-1 (diagonal of the strip's first row)
-    float dtMM = __fmul_rn((float)(-i0), P.egq), dtDG = HHG_NEG, dtMI = HHG_NEG, dtGD = HHG_NEG,
-          dtIM = HHG_NEG;
+    float dtMM = __fmul_rn((float)(-i0), P.egq), dtDG = HHG_NEG, dtGD = HHG_NEG, dtIM = HHG_NEG;
 
     float best = HHG_NEG;
     int bi = 0, bj = 0;
@@ -275,10 +282,12 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
     // boundary values of column 1 (strips > 0): issue the slot load now, validate the tag at use
     float nMM = 0.f, nDG = 0.f, nMI = 0.f, nGD = 0.f, nIM = 0.f;
     uint32_t ntag[5] = {0u, 0u, 0u, 0u, 0u};
-    if (s > 0) ld_slot(bnd + 32, lane, nMM, nDG, nMI, nGD, nIM, ntag);
+    if (s > 0) ld_slot(bndc, lane, nMM, nDG, nMI, nGD, nIM, ntag);
 
     mbar_wait(bar, parity);
     parity ^= 1u;
+#pragma unroll
+    for (int r = 0; r < R; ++r) Y[r] = __fadd_rn(HHG_NEG, qs[r * 7 + 5].x);   // MI(., 0) = -FLT_MAX
 
     for (int j = 1; j <= Lmax; ++j) {
       // ---- current column operands (from the prefetch registers), prefetch the next column
@@ -286,31 +295,35 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
       const float t_m2m = nx[5].x, t_m2d = nx[5].y, t_d2m = nx[5].z, t_d2d = nx[5].w;
       const float t_i2m = nx[6].x, t_i2i = nx[6].y, t_m2i = nx[6].z;
       const uint32_t t_ss = __float_as_uint(nx[6].w);
-      {
-        const float4* src = jc + (size_t)(min(j + 1, Lmax) - 1) * 224;
+      jc += 224;
 #pragma unroll
-        for (int k = 0; k < 7; ++k) nx[k] = ld_jc(src + k * 32);
-      }
+      for (int k = 0; k < 7; ++k) nx[k] = ld_jc(jc + k * 32);
 
-      // ---- boundary row i0 at column j: slot prefetched during column j-1; spin (per lane) until the
-      // producer strip's tag is there, then prefetch column j+1
+      // ---- boundary row i0 at column j: slot prefetched during column j-1; wait until the producer strip's
+      // tag is there, then prefetch column j+1
       float tMM, tDG, tMI, tGD, tIM;
       if (s == 0) {
         tMM = __fmul_rn((float)(-j), P.egt);   // :148
         tDG = tMI = tGD = tIM = HHG_NEG;
       } else {
-        // all five words must carry the producer's tag
-        while (!slot_ok(ntag, tag_in)) {
-          __nanosleep(20);
-          ld_slot(bnd + (size_t)j * 32, lane, nMM, nDG, nMI, nGD, nIM, ntag);
+        // all five words must carry the producer's tag.  One warp vote on the common path; strip s-1 normally runs
+        // ahead, so the per-lane retry loop is rare
+        if (!__all_sync(0xffffffffu, slot_ok(ntag, tag_in))) {
+          while (!slot_ok(ntag, tag_in)) {
+            __nanosleep(20);
+            ld_slot(bndc, lane, nMM, nDG, nMI, nGD, nIM, ntag);
+          }
         }
         tMM = nMM; tDG = nDG; tMI = nMI; tGD = nGD; tIM = nIM;
-        if (j < Lmax) ld_slot(bnd + (size_t)(j + 1) * 32, lane, nMM, nDG, nMI, nGD, nIM, ntag);
+        ld_slot(bndc + 32, lane, nMM, nDG, nMI, nGD, nIM, ntag);
       }
       uint32_t cow = 0;
-      if (CELLOFF) cow = __ldg(co + (size_t)j * 32);
+      if (CELLOFF) cow = __ldg(co);
 
-      float dMM = dtMM, dGD = dtGD, dIM = dtIM, dDG = dtDG, dMI = dtMI;   // cell (i-1, j-1)
+      // row 0's diagonal partial sums from the boundary row at column j-1; row r+1's are formed by row r
+      float4 qa = qs[5], qb = qs[6];
+      float pMM = __fadd_rn(dtMM, qa.x), pGD = __fadd_rn(dtGD, qa.x), pIM = __fadd_rn(dtIM, qb.x),
+            pDG = __fadd_rn(dtDG, qa.z);
       float uMM = tMM, uDG = tDG, uMI = tMI;                              // cell (i-1, j)
       const float bcmp = (j <= Lt) ? best : INFINITY;   // padded columns never become the maximum
       float bc = bcmp;
@@ -322,20 +335,17 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
         float4 q[5];
 #pragma unroll
         for (int k = 0; k < 5; ++k) q[k] = qs[r * 7 + k];
-        const float4 qa = qs[r * 7 + 5], qb = qs[r * 7 + 6];
         const float q_m2m = qa.x, q_m2d = qa.y, q_d2m = qa.z, q_d2d = qa.w;
         const float q_i2m = qb.x, q_i2i = qb.y, q_m2i = qb.z;
-
-        const float oMM = MM[r], oGD = GD[r], oIM = IM[r], oDG = DG[r], oMI = MI[r];   // (i, j-1)
 
         // 5-way maximum with the reference's strict-'>' / first-wins rule, :241-273
         uint32_t b;
         float mm;
-        const float c1 = __fadd_rn(__fadd_rn(dMM, q_m2m), t_m2m);
-        const float c2 = __fadd_rn(__fadd_rn(dGD, q_m2m), t_d2m);
-        const float c3 = __fadd_rn(__fadd_rn(dIM, q_i2m), t_m2m);
-        const float c4 = __fadd_rn(__fadd_rn(dDG, q_d2m), t_m2m);
-        const float c5 = __fadd_rn(__fadd_rn(dMI, q_m2m), t_i2m);
+        const float c1 = __fadd_rn(pMM, t_m2m);     // (MM(i-1,j-1) + q_m2m) + t_m2m
+        const float c2 = __fadd_rn(pGD, t_d2m);     // (GD(i-1,j-1) + q_m2m) + t_d2m
+        const float c3 = __fadd_rn(pIM, t_m2m);     // (IM(i-1,j-1) + q_i2m) + t_m2m
+        const float c4 = __fadd_rn(pDG, t_m2m);     // (DG(i-1,j-1) + q_d2m) + t_m2m
+        const float c5 = __fadd_rn(Y[r], t_i2m);    // (MI(i-1,j-1) + q_m2m) + t_i2m
 #if HHG_MAX3
         // the winner of the strict-'>' chain is the FIRST candidate (order STOP, MM, GD, IM, DG, MI) that attains
         // the maximum: five maxima + five equality selects instead of five max + five '>' selects
@@ -364,6 +374,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
         Si = __fadd_rn(Si, P.shift);                                   // :281
         mm = __fadd_rn(mm, Si);
 
+        const float oMM = MM[r], oGD = GD[r], oIM = IM[r], oDG = DG[r];   // (i, j-1)
         float a1, a2, gd, im, dg, mi;
         a1 = __fadd_rn(oMM, t_m2d); a2 = __fadd_rn(oGD, t_d2d);                                // :307
         b |= (a1 > a2) ? 8u : 0u;  gd = fmaxf(a1, a2);
@@ -371,7 +382,8 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
         b |= (a1 > a2) ? 16u : 0u; im = fmaxf(a1, a2);
         a1 = __fadd_rn(uMM, q_m2d); a2 = __fadd_rn(uDG, q_d2d);                                // :340
         b |= (a1 > a2) ? 32u : 0u; dg = fmaxf(a1, a2);
-        a1 = __fadd_rn(__fadd_rn(uMM, q_m2m), t_m2i); a2 = __fadd_rn(__fadd_rn(uMI, q_m2m), t_i2i);   // :358
+        Y[r] = __fadd_rn(uMI, q_m2m);                                                           // c5 of column j+1
+        a1 = __fadd_rn(__fadd_rn(uMM, q_m2m), t_m2i); a2 = __fadd_rn(Y[r], t_i2i);             // :358
         b |= (a1 > a2) ? 64u : 0u; mi = fmaxf(a1, a2);
 
         if (CELLOFF) {                                                 // :373-392
@@ -382,15 +394,20 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
 
         word |= b << (8 * (r & 3));
         if ((r & 3) == 3) {
-          __stcs(btj + (size_t)((i0 >> 2) + (r >> 2)) * bt_row_stride + (size_t)j * 32, word);
+          __stcs(btc + (size_t)(r >> 2) * bt_row_stride, word);
           word = 0;
         }
-        // rotate: this row's old values are the next row's diagonal, its new values the next row's up
-        dMM = oMM; dGD = oGD; dIM = oIM; dDG = oDG; dMI = oMI;
+        // the next row's diagonal partial sums, from this row's old values before they are overwritten
+        if (r + 1 < R) {
+          qa = qs[(r + 1) * 7 + 5]; qb = qs[(r + 1) * 7 + 6];
+          pMM = __fadd_rn(oMM, qa.x); pGD = __fadd_rn(oGD, qa.x); pIM = __fadd_rn(oIM, qb.x);
+          pDG = __fadd_rn(oDG, qa.z);
+        }
+        // this row's new values are the next row's up
         uMM = mm; uDG = dg; uMI = mi;
-        MM[r] = mm; GD[r] = gd; IM[r] = im; DG[r] = dg; MI[r] = mi;
+        MM[r] = mm; GD[r] = gd; IM[r] = im; DG[r] = dg;
       }
-      dtMM = tMM; dtDG = tDG; dtMI = tMI; dtGD = tGD; dtIM = tIM;
+      dtMM = tMM; dtDG = tDG; dtGD = tGD; dtIM = tIM;
 
       // running maximum, :423-455: ONE test per column on the maximum of the R new MM values (a tree of
       // FMNMX, 1 instruction per row instead of compare+branch per cell); only when it can matter the
@@ -415,8 +432,10 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
         }
       }
 
-      if (!last_strip)
-        st_slot(bnd + (size_t)j * 32, lane, MM[R - 1], DG[R - 1], MI[R - 1], GD[R - 1], IM[R - 1], tag_out);
+      if (!last_strip) st_slot(bndc, lane, uMM, uDG, uMI, GD[R - 1], IM[R - 1], tag_out);
+      bndc += 32;
+      btc += 32;
+      if (CELLOFF) co += 32;
     }
     const size_t o = ((size_t)P.job_ss_off[job] + s) * 32 + lane;
     P.strip_score[o] = best;
