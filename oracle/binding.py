@@ -443,6 +443,25 @@ class RefShim:
                     j=oj[:nn + 1].copy(), states=st, P_posterior=ops[:nn + 1].copy(), post=post, t_tr_lin=ttl,
                     q_tr_lin=qtl)
 
+    def mac_forward_only(self, t_p, t_tr, vit, local=True, shift=-0.03):
+        """PosteriorDecoder::forwardAlgorithm alone, set up like mac_realign (no exclusions): the row scale factors
+        scale[0..Lq+1], Pforward and the forward matrix as stored before the backward pass overwrites it."""
+        Lq = self.Lq
+        Lt = t_p.shape[0] - 2
+        if Lt + 2 > self.maxres or Lq + 2 > self.maxres:
+            raise ValueError(f"Lq={Lq}, Lt={Lt} exceed maxres {self.maxres}")
+        t_p = np.ascontiguousarray(t_p, np.float32); t_tr = np.ascontiguousarray(t_tr, np.float32)
+        i1, i2, j1, j2, n, vi, vj = vit
+        vi = np.ascontiguousarray(vi, np.int32); vj = np.ascontiguousarray(vj, np.int32)
+        fwd = np.zeros((Lq + 1, Lt + 1), np.float32); scale = np.zeros(Lq + 2, np.float64); pf = C.c_double()
+        dp = C.POINTER(C.c_double)
+        self.lib.hhref_mac_forward_only.argtypes = [C.c_int, c_f32p, c_f32p, C.c_int, C.c_float, C.c_int, C.c_int,
+                                                    C.c_int, C.c_int, C.c_int, c_i32p, c_i32p, c_f32p, dp, dp]
+        self.lib.hhref_mac_forward_only(Lt, _p(t_p, c_f32p), _p(t_tr, c_f32p), 1 if local else 0, shift, i1, i2, j1, j2,
+                                        n, _p(vi, c_i32p), _p(vj, c_i32p), _p(fwd, c_f32p), scale.ctypes.data_as(dp),
+                                        C.byref(pf))
+        return dict(scale=scale, Pforward=pf.value, fwd=fwd)
+
     def fast_log2_table(self):
         """lg2[0..1024] of the reference's fast_log2 (x in [1,2): a=0, c=0 -> returns lg2[b] exactly)."""
         x = ((np.arange(1024, dtype=np.uint32) << 13) | np.uint32(0x3F800000)).view(np.float32)

@@ -3,6 +3,7 @@ reference: committed goldens, and the compiled reference on fresh cases when it 
 import numpy as np
 import pytest
 
+from tests import mac_cases as mc
 from tests.util import bits, golden
 
 
@@ -68,6 +69,55 @@ def test_oracle_mac_equals_compiled_reference(oracle, refshim, seed):
                 m2 = oracle.mac_realign(qp, qlin, tp, oracle.log2lin(ttr), vit, excl=ex, local=local, mact=mact)
                 assert r2["Pforward"] == m2["Pforward"] and np.array_equal(r2["i"][1:], m2["i"][1:])
                 assert np.array_equal(bits(r2["post"][1:, 1:]), bits(m2["post"][1:, 1:]))
+
+
+# Lq -> template lengths: every query length crossed with some of the launch-boundary lengths (tests/mac_cases.py), so
+# that every boundary length and every query length appears at least once.
+LONG_CASES = {1: (1, mc.LARGE_MIN, mc.FALLBACK_MIN), 2: (1, mc.SMALL_MAX, mc.LONG_LT),
+              700: (mc.SMALL_MAX, mc.LARGE_MIN, mc.WINDOW_MAX, mc.FALLBACK_MIN), 1500: (1, mc.WINDOW_MAX, mc.LONG_LT)}
+
+
+def _oracle_mac(oracle, qp, qtr, t, vit, **kw):
+    return oracle.mac_realign(qp, oracle.log2lin(qtr), t[0], oracle.log2lin(t[1]), vit, **kw)
+
+
+@pytest.mark.parametrize("Lq", sorted(LONG_CASES))
+def test_oracle_mac_equals_compiled_reference_long(oracle, refshim, Lq):
+    """Queries of 1, 2, 700 and 1500 columns against templates at the shared-memory window boundaries and beyond, with
+    the homology in the middle of the template; every mode, then a second alignment with the first one excluded."""
+    from hhsuite_b200 import synth
+    rng = np.random.default_rng(1000 + Lq)
+    qp, qtr, qss, qpav, qcols = synth.query_profile(Lq, 40 + Lq)
+    refshim.set_query(qp, qtr, qpav, None)
+    for Lt in LONG_CASES[Lq]:
+        t = mc.embedded(Lt, qcols, rng, noise=0.2)
+        vit = mc.ref_viterbi(refshim, t[0], t[1])
+        assert vit is not None, (Lq, Lt)
+        for local, mact in mc.MODES:
+            what = (Lq, Lt, local, mact)
+            ref = refshim.mac_realign(t[0], t[1], vit, local=local, mact=mact)
+            mc.assert_same(ref, _oracle_mac(oracle, qp, qtr, t, vit, local=local, mact=mact), what)
+            if ref["nsteps"] > 0:
+                ex = [(ref["i"][1:], ref["j"][1:])]
+                r2 = refshim.mac_realign(t[0], t[1], vit, excl=ex, local=local, mact=mact)
+                mc.assert_same(r2, _oracle_mac(oracle, qp, qtr, t, vit, excl=ex, local=local, mact=mact), what + ("excl",))
+
+
+def test_oracle_mac_underflow_clamp_equals_compiled_reference(oracle, refshim):
+    """A near-self hit of 1500 columns accumulates enough forward mass that the product of the row scale factors falls
+    below DBL_MIN*100, so the forward and backward clamp branches run; the oracle still matches bit for bit."""
+    Lq = 1500
+    (qp, qtr, qss, qpav, qcols), t = mc.near_self(Lq, 78)
+    refshim.set_query(qp, qtr, qpav, None)
+    vit = mc.ref_viterbi(refshim, t[0], t[1])
+    assert vit[4] > Lq // 2
+    fw = refshim.mac_forward_only(t[0], t[1], vit)
+    row = mc.first_clamped_row(fw["scale"], Lq)
+    assert row is not None and row < 2 * Lq // 3, row
+    assert fw["Pforward"] == refshim.mac_realign(t[0], t[1], vit, want_post=False)["Pforward"]
+    for local, mact in mc.MODES:
+        ref = refshim.mac_realign(t[0], t[1], vit, local=local, mact=mact)
+        mc.assert_same(ref, _oracle_mac(oracle, qp, qtr, t, vit, local=local, mact=mact), (local, mact))
 
 
 def test_host_log2lin_equals_oracle(oracle):

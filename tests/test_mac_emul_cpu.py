@@ -1,7 +1,9 @@
 """The product's MAC kernels (hh-suite_b200/csrc/hhg_mac.cuh, unmodified source) executed on the CPU by the host
 emulation in tests/emul/ (one OS thread per CUDA thread, barriers for __syncwarp, an exchange buffer for shuffles) and
 compared bit for bit with the oracle.  This is how kernel changes are checked in the authoring container before GPU
-minutes are spent; it also exercises paths the GPU tests rarely hit (global-scratch fallback, band-limited scans)."""
+minutes are spent.  Both scan modes run (HHG_MAC_BANDSCAN: band-limited scans by default, full-row scans with 0), and
+smem=0 forces the global-scratch fallback on short inputs, which the GPU only takes for templates longer than 1747
+columns (tests/mac_cases.py)."""
 import ctypes as C
 import os
 import subprocess
@@ -35,7 +37,7 @@ def emul():
     return L
 
 
-def _run(L, oracle, qp, qlin, tp, ttr, vit, excl=None, local=True, shift=-0.03, mact=0.35, smem=64 * 1024, band=0):
+def _run(L, oracle, qp, qlin, tp, ttr, vit, excl=None, local=True, shift=-0.03, mact=0.35, smem=64 * 1024, band=1):
     Lq, Lt = qp.shape[0] - 2, tp.shape[0] - 2
     i1, i2, j1, j2, n, vi, vj = vit
     v5 = np.array([i1, i2, j1, j2, n], np.int32)
@@ -92,7 +94,7 @@ FULL = os.environ.get("HHG_EMUL_FULL") == "1"      # the extended sweep (minutes
 @pytest.mark.parametrize("seed", [1, 2] if FULL else [1])
 @pytest.mark.parametrize("band", [0, 1])
 def test_emulated_kernel_equals_oracle(emul, oracle, seed, band):
-    """band=0: the shipped kernel path; band=1: the band-limited scans (opt-in HHG_MAC_BANDSCAN=1).  Shared-memory
+    """band=1: the band-limited scans, the default; band=0: the full-row scans (HHG_MAC_BANDSCAN=0).  Shared-memory
     working set and the global-scratch fallback (smem=0), local/global mode, several mact, a second alignment."""
     configs = ((True, 0.35, 64 * 1024), (True, 0.0, 0), (False, 0.1, 64 * 1024)) if FULL else \
         ((True, 0.35, 64 * 1024), (False, 0.1, 0))

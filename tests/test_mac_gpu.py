@@ -1,9 +1,12 @@
 """GPU parity of the MAC realignment (hhg_mac_realign, SURVEY 8f-3) through the C-ABI: posterior matrix, Pforward, MAC
 path and per-step posteriors must be bit-identical to the reference (goldens; compiled reference when shipped) and to
 the oracle's restatement, for local/global mode, several mact thresholds and alternative alignments."""
+import functools
+
 import numpy as np
 import pytest
 
+from tests import mac_cases as mc
 from tests.util import bits, golden
 
 pytestmark = pytest.mark.gpu
@@ -211,4 +214,199 @@ def test_mac_error_paths(hhg, gpu_ctx):
         hhg.capi.mac_realign(gpu_ctx, db, [0], [(1, 5, 1, 45, 5, np.arange(6), np.arange(6))])
     with pytest.raises(hhg.HhgError, match="leaves the matrix"):
         hhg.capi.mac_realign(gpu_ctx, db, [0], [(1, 5, 1, 5, 5, np.arange(6), np.arange(6) + 40)])
+    db.close()
+
+
+# --------------------------------------------------------------------------- long queries and templates
+# hhg_mac_realign runs a request in one of three places chosen from its template length (tests/mac_cases.py): the 64 KiB
+# shared-memory launch on the context's stream, the 200 KiB launch on the auxiliary stream (requests mapped through
+# req_map), or the global row scratch inside that second launch.  The tests below put requests on both sides of each
+# boundary, in one call and in single-class calls, and compare every request with the oracle.
+def _oracle_mac(oracle, q, t, vit, local, mact, excl=()):
+    return oracle.mac_realign(q[0], oracle.log2lin(q[1]), t[0], oracle.log2lin(t[1]), vit, excl=excl, local=local,
+                              mact=mact)
+
+
+def _gpu_vits(hhg, ctx, db):
+    """{target: Viterbi (i1, i2, j1, j2, nsteps, i_steps, j_steps)} of every target with a non-empty path."""
+    hits, paths = hhg.viterbi_search(ctx, db)
+    out = {}
+    for t in range(db.n):
+        ns = int(hits["nsteps"][t])
+        if ns:
+            i_s, j_s, _ = hhg.expand_path(hits[t], paths)
+            out[t] = (int(hits["i1"][t]), int(hits["i2"][t]), int(hits["j1"][t]), int(hits["j2"][t]), ns, i_s, j_s)
+    return out
+
+
+def _mac_checked(hhg, ctx, db, oracle, q, tg, ids, vits, local, mact):
+    """One hhg_mac_realign call over `ids`; every request (hit fields, path, per-step posteriors, posterior matrix)
+    against the oracle, all mismatching requests reported together.  Returns the number of kernel launches the call
+    made."""
+    before = ctx.launches
+    mh, mp = hhg.capi.mac_realign(ctx, db, ids, [vits[t] for t in ids], local=local, mact=mact)
+    launches = ctx.launches - before
+    bad = []
+    for r, t in enumerate(ids):
+        Lt = tg[t][0].shape[0] - 2
+        got = {f: int(mh[f][r]) for f in ("i1", "i2", "j1", "j2", "nsteps", "matched_cols")}
+        got.update(Pforward=float(mh["pforward"][r]), sum_of_probs=mh["sum_of_probs"][r], i=mp[r]["i"], j=mp[r]["j"],
+                   states=mp[r]["states"], P_posterior=mp[r]["P_posterior"], post=hhg.capi.mac_debug_posterior(ctx, r, Lt))
+        try:
+            mc.assert_same(_oracle_mac(oracle, q, tg[t], vits[t], local, mact), got, (r, t, Lt, local, mact))
+        except AssertionError as e:
+            bad.append(e.args[0] if e.args else (r, t, Lt))
+    assert not bad, bad
+    return launches
+
+
+def _is_large(Lt):
+    return mc.need(Lt) > mc.SMALL_WINDOW
+
+
+@functools.lru_cache(maxsize=None)
+def _long_case():
+    """Lq = 1200 against a homolog at every boundary length and one unrelated template, in an order where small and
+    large requests interleave."""
+    from hhsuite_b200 import synth
+    rng = np.random.default_rng(2024)
+    q = synth.query_profile(1200, 61)
+    tg = [mc.embedded(L, q[4], rng) for L in mc.BOUNDARY_LENGTHS] + [synth.prepared_profile(800, rng)]
+    order = [2, 0, 5, 3, 1, 6, 4]       # 558, 1, 3000, 1747, 557, 800 (unrelated), 1748
+    return q, [tg[k] for k in order]
+
+
+@pytest.mark.parametrize("local,mact", mc.MODES)
+def test_mac_long_mixed_call(hhg, gpu_ctx, oracle, local, mact):
+    """One call holding requests of all three kinds: two launches on two streams, the large one reading its requests
+    through req_map.  The small-only and large-only calls of the same requests make one launch fewer."""
+    q, tg = _long_case()
+    gpu_ctx.set_query(q[0], q[1])
+    db = hhg.TargetDB.from_profiles(gpu_ctx, tg)
+    vits = _gpu_vits(hhg, gpu_ctx, db)
+    ids = sorted(vits)
+    assert len(ids) == len(tg)
+    large = [_is_large(tg[t][0].shape[0] - 2) for t in ids]
+    assert any(large) and not all(large) and large != sorted(large)    # req_map is not the identity
+    hhg.capi.mac_query_set(gpu_ctx, q[0], hhg.capi.log2lin(q[1]))
+    mixed = _mac_checked(hhg, gpu_ctx, db, oracle, q, tg, ids, vits, local, mact)
+    small_only = _mac_checked(hhg, gpu_ctx, db, oracle, q, tg, [t for t, b in zip(ids, large) if not b], vits, local, mact)
+    large_only = _mac_checked(hhg, gpu_ctx, db, oracle, q, tg, [t for t, b in zip(ids, large) if b], vits, local, mact)
+    assert mixed == small_only + 1 and large_only == small_only, (mixed, small_only, large_only)
+    db.close()
+
+
+@pytest.mark.parametrize("lens,local,mact", [((mc.LARGE_MIN, mc.WINDOW_MAX), True, 0.35),
+                                             ((mc.FALLBACK_MIN, mc.LONG_LT), False, 0.1),
+                                             ((mc.WINDOW_MAX, mc.FALLBACK_MIN, mc.LARGE_MIN, mc.LONG_LT), True, 0.0)],
+                         ids=["window", "fallback", "window+fallback"])
+def test_mac_long_single_class(hhg, gpu_ctx, oracle, lens, local, mact):
+    """Calls with no small request: only requests inside the 200 KiB window, only global-scratch requests, and one
+    large launch holding both."""
+    q, tg = _long_case()
+    gpu_ctx.set_query(q[0], q[1])
+    db = hhg.TargetDB.from_profiles(gpu_ctx, tg)
+    vits = _gpu_vits(hhg, gpu_ctx, db)
+    by_len = {tg[t][0].shape[0] - 2: t for t in vits}
+    ids = [by_len[L] for L in lens]
+    hhg.capi.mac_query_set(gpu_ctx, q[0], hhg.capi.log2lin(q[1]))
+    _mac_checked(hhg, gpu_ctx, db, oracle, q, tg, ids, vits, local, mact)
+    db.close()
+
+
+def test_mac_underflow_clamp_against_compiled_reference(hhg, gpu_ctx, refshim):
+    """The near-self Lq = 1500 hit whose forward scale product falls below DBL_MIN*100 (both clamp branches run), in
+    the 200 KiB window, against the compiled reference."""
+    Lq = 1500
+    (qp, qtr, qss, qpav, qcols), t = mc.near_self(Lq, 78)
+    refshim.set_query(qp, qtr, qpav, None)
+    vit = mc.ref_viterbi(refshim, t[0], t[1])
+    assert mc.first_clamped_row(refshim.mac_forward_only(t[0], t[1], vit)["scale"], Lq) < Lq
+    gpu_ctx.set_query(qp, qtr)
+    db = hhg.TargetDB.from_profiles(gpu_ctx, [t])
+    hhg.capi.mac_query_set(gpu_ctx, qp, hhg.capi.log2lin(qtr))
+    for local, mact in mc.MODES:
+        ref = refshim.mac_realign(t[0], t[1], vit, local=local, mact=mact)
+        mh, mp = hhg.capi.mac_realign(gpu_ctx, db, [0], [vit], local=local, mact=mact)
+        _check(mh[0], mp[0], ref)
+        post = hhg.capi.mac_debug_posterior(gpu_ctx, 0, Lq)
+        assert np.array_equal(bits(post[1:, 1:]), bits(ref["post"][1:, 1:])), (local, mact)
+    db.close()
+
+
+@pytest.mark.parametrize("Lq", [1, 2])
+def test_mac_query_of_one_or_two_columns(hhg, gpu_ctx, oracle, Lq):
+    """Lq = 1 skips the forward row loop and the backward row loop; Lq = 2 runs each once.  Short templates, a
+    window-sized one and a global-scratch one, in one call."""
+    from hhsuite_b200 import synth
+    rng = np.random.default_rng(300 + Lq)
+    q = synth.query_profile(Lq, 90 + Lq)
+    tg = [mc.embedded(L, q[4], rng) for L in (1, 2, 60, 600, mc.FALLBACK_MIN + 52)]
+    gpu_ctx.set_query(q[0], q[1])
+    db = hhg.TargetDB.from_profiles(gpu_ctx, tg)
+    vits = _gpu_vits(hhg, gpu_ctx, db)
+    assert sorted(vits) == list(range(len(tg)))
+    hhg.capi.mac_query_set(gpu_ctx, q[0], hhg.capi.log2lin(q[1]))
+    for local, mact in mc.MODES:
+        _mac_checked(hhg, gpu_ctx, db, oracle, q, tg, sorted(vits), vits, local, mact)
+    db.close()
+
+
+def test_mac_alternative_alignments_fallback(hhg, gpu_ctx, oracle):
+    """mac.realign's exclusion rounds on templates with two copies of the query: one longer than the 200 KiB window
+    (global scratch), one inside it."""
+    from hhsuite_b200 import synth
+    rng = np.random.default_rng(17)
+    Lq = 300
+    q = synth.query_profile(Lq, 33)
+    qp, qtr = q[0], q[1]
+    tg = [mc.two_copies(Lq, mc.FALLBACK_MIN + 152, q[4], rng), mc.two_copies(Lq, 1000, q[4], rng)]
+    gpu_ctx.set_query(qp, qtr)
+    db = hhg.TargetDB.from_profiles(gpu_ctx, tg)
+    vhits = hhg.runner.ViterbiRunner(gpu_ctx, db, altali=3, smin=20.0).alignment()
+    vhits = [h for h in vhits if h.nsteps > 0]
+    for t in range(len(tg)):
+        assert max(h.irep for h in vhits if h.target == t) >= 2, t
+    got = hhg.mac.realign(gpu_ctx, db, qp, qtr, vhits, mact=0.35)
+    assert set(got) == {(h.target, h.irep) for h in vhits}
+    by_t = {}
+    for h in sorted(vhits, key=lambda h: (h.target, h.irep)):
+        by_t.setdefault(h.target, []).append(h)
+    for t, hs in by_t.items():
+        alt_i, alt_j = [], []
+        for h in hs:
+            ex = [(np.array(alt_i, np.int32), np.array(alt_j, np.int32))] if alt_i else ()
+            want = _oracle_mac(oracle, q, tg[t], (h.i1, h.i2, h.j1, h.j2, h.nsteps, h.i, h.j), True, 0.35, ex)
+            m = got[(t, h.irep)]
+            assert (m.i1, m.i2, m.j1, m.j2, m.nsteps, m.matched_cols) == tuple(want[f] for f in ("i1", "i2", "j1", "j2", "nsteps", "matched_cols"))
+            assert m.pforward == want["Pforward"]
+            n = want["nsteps"]
+            assert np.array_equal(m.i[1:], want["i"][1:n + 1]) and np.array_equal(m.j[1:], want["j"][1:n + 1])
+            assert np.array_equal(bits(m.P_posterior[1:]), bits(want["P_posterior"][1:n + 1]))
+            if n:
+                alt_i += want["i"][1:n + 1].tolist(); alt_j += want["j"][1:n + 1].tolist()
+            else:
+                alt_i.append(want["i2"]); alt_j.append(want["j2"])
+    db.close()
+
+
+def test_mac_short_call_after_long_call(hhg, gpu_ctx, oracle):
+    """Scratch reuse on one context: a long call (global-scratch requests) leaves larger, dirty buffers behind; a short
+    call that follows, and its posterior matrices, still equal the oracle."""
+    from hhsuite_b200 import synth
+    q, tg = _long_case()
+    gpu_ctx.set_query(q[0], q[1])
+    db = hhg.TargetDB.from_profiles(gpu_ctx, tg)
+    vits = _gpu_vits(hhg, gpu_ctx, db)
+    hhg.capi.mac_query_set(gpu_ctx, q[0], hhg.capi.log2lin(q[1]))
+    hhg.capi.mac_realign(gpu_ctx, db, sorted(vits), [vits[t] for t in sorted(vits)], mact=0.0)
+    db.close()
+    rng = np.random.default_rng(5)
+    qs = synth.query_profile(90, 8)
+    ts = [synth.prepared_profile(L, rng, qs[4] if k != 1 else None, noise=0.2) for k, L in enumerate((90, 40, 130, 1))]
+    gpu_ctx.set_query(qs[0], qs[1])
+    db = hhg.TargetDB.from_profiles(gpu_ctx, ts)
+    vs = _gpu_vits(hhg, gpu_ctx, db)
+    hhg.capi.mac_query_set(gpu_ctx, qs[0], hhg.capi.log2lin(qs[1]))
+    _mac_checked(hhg, gpu_ctx, db, oracle, qs, ts, sorted(vs), vs, True, 0.35)
     db.close()
