@@ -1468,10 +1468,13 @@ int hhg_set_use_ss(hhg_ctx* ctx, int use_ss) {
 }
 
 // ---------------------------------------------------------------------------------------- plan
-// Strip height of a plan.  Whole-shard scans have work items to spare and take R = 16 (least per-column overhead,
-// 253 GCUPS).  A small request (the few thousand survivors of the prefilter) is latency bound: its longest job is one
-// serial sweep over Lmax columns per strip, so halving the strip height halves that critical path and doubles the
-// number of work items that can run side by side.
+// Strip height of a plan.  Whole-shard scans have work items to spare and take R = 16: the least per-column overhead
+// (boundary hand-off, operand copies, running maximum) per row.  R = 12 fits 3 CTAs per SM instead of 2 but measures
+// slower on an H100 (400 W limit, SM clock 1.59-1.64 GHz): 61.8-62.8 ms against 55.6-55.8 ms per launch at Lq = 400
+// (34 strips of 12, 2 % padded rows) and 55.9-56.2 against 55.5-55.7 ms at Lq = 1500 (tools/vit_ab.py).
+// A small request (the few thousand survivors of the prefilter) is latency bound: its longest job is one serial sweep
+// over Lmax columns per strip, so halving the strip height halves that critical path and doubles the number of work
+// items that can run side by side.
 static int plan_strip_rows(const hhg_ctx* ctx, const int32_t* req_query, int n) {
   if (ctx->R) return ctx->R;
   long long items16 = 0;
@@ -1763,7 +1766,8 @@ int hhg_set_excluded_regions(hhg_ctx* ctx, int nq, const int32_t* q_lo, const in
 
 template <int R>
 static int launch_viterbi(hhg_ctx* ctx, const VitParams& P, bool local, bool ss, bool co, int items) {
-  const size_t smem = (size_t)kWarpsPerCta * R * 112 + 64 + (ss ? 44 * 44 * 4 : 0);
+  // per warp: R query rows and the two-column operand ring; then the mbarriers and the S33 table
+  const size_t smem = (size_t)kWarpsPerCta * (R * 112 + kRingBytes) + 64 + (ss ? 44 * 44 * 4 : 0);
   void (*kern)(const VitParams) = nullptr;
 #define PICK(L_, S_, C_) kern = k_viterbi<R, L_, S_, C_>
   if (local) { if (ss) { if (co) PICK(true, true, true); else PICK(true, true, false); }

@@ -17,7 +17,10 @@
 //   * target operands stream from a JOB-INTERLEAVED copy of the job's column records,
 //     [column][k = 0..6][lane] float4 (built per plan by k_interleave_cols), so each of the 7 loads of a
 //     column is ONE coalesced 512-byte warp request (4 L1TEX wavefronts instead of 32 when every lane
-//     reads its own 112-byte record), register-prefetched one column ahead.
+//     reads its own 112-byte record).  Lane l only ever touches the elements [k][l], so every lane cp.asyncs its own
+//     7 x 16 B of column j+1 into a lane-private slot of a two-column shared-memory ring while column j computes, and
+//     reads them back with its own LDS.128 after its own cp.async.wait_group: no barrier, no elected lane, no
+//     cross-lane ordering, and no registers held for the next column.
 //   * 1 backtrace byte per cell, packed 4 rows per 32-bit word and stored lane-interleaved so
 //     every warp store writes one full 128-byte line.
 // Arithmetic is the reference's, operation for operation (unfused fp32 mul/add in the same order,
@@ -187,8 +190,17 @@ __device__ __forceinline__ float dot20_dev(const float4 (&t)[5], const float4 (&
   return __fadd_rn(__fadd_rn(r0, r1), __fadd_rn(r2, r3));
 }
 
-// one 16-byte operand of the job-interleaved stream: L2-only load (a line is read once per strip and SM)
-__device__ __forceinline__ float4 ld_jc(const float4* p) { return __ldcg(p); }
+// one 16-byte operand of the job-interleaved stream into this thread's ring slot: L2 only (a line is read once per
+// strip and SM).  The data is visible to the issuing thread after its cp.async.wait_group.
+__device__ __forceinline__ void cp_async_jc(float4* dst, const float4* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// operand ring of one warp: 2 column slots x 7 operands x 32 lanes (float4), i.e. one column in flight
+constexpr int kJcSlot = 7 * 32;                 // float4 per column slot
+constexpr size_t kRingBytes = 2 * kJcSlot * 16;   // 7168 B per warp
 
 #define HHG_NEG (-FLT_MAX)
 
@@ -203,9 +215,12 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  // smem carve-up: [warps][R] query records | mbarriers | (SS) the S33 table
+  // smem carve-up: [warps][R] query records | [warps] operand rings | mbarriers | (SS) the S33 table
   float4* qs = reinterpret_cast<float4*>(smem_raw) + (size_t)warp * R * 7;
-  constexpr size_t kBarOff = (size_t)kWarpsPerCta * R * 112;
+  constexpr size_t kRingOff = (size_t)kWarpsPerCta * R * 112;
+  // this lane's elements of the warp's ring: operand k of slot x at ring[x * kJcSlot + k * 32]
+  float4* ring = reinterpret_cast<float4*>(smem_raw + kRingOff + (size_t)warp * kRingBytes) + lane;
+  constexpr size_t kBarOff = kRingOff + kWarpsPerCta * kRingBytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + kBarOff);
   float* s33 = reinterpret_cast<float*>(smem_raw + kBarOff + 64);
   uint64_t* bar = bars + warp;
@@ -244,8 +259,8 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
     const int Lt = P.Lt[t];
     const int Lmax = P.job_Lmax[job];
     // per-column pointers advance by constants: the operand stream by 7 x 32 float4, slots and backtrace words by 32.
-    // The plan allocates one column of slack after the last job's stream and slots, so the prefetch of column j+1
-    // needs no clamp (what it reads after the job's last column is never used)
+    // The plan allocates one column of slack after the last job's stream and slots, so the copy of column j+1 into
+    // the ring needs no clamp (what it reads after the job's last column is never used)
     const float4* jc = P.jcols + P.job_jc_off[job] + lane;   // operand k of the prefetched column: jc[k*32]
     const size_t bt_row_stride = (size_t)(Lmax + 1) * 32;   // words per 4-row group
     uint32_t* btc = P.bt + P.job_bt_off[job] + lane + (size_t)(i0 >> 2) * bt_row_stride + 32;   // column j
@@ -274,10 +289,11 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
     float best = HHG_NEG;
     int bi = 0, bj = 0;
 
-    // first column (register prefetch, one column ahead); L2-only loads: a line is read once per strip
-    float4 nx[7];
+    // first column into ring slot 0 (Lmax >= 1); column j lives in slot (j - 1) & 1
 #pragma unroll
-    for (int k = 0; k < 7; ++k) nx[k] = ld_jc(jc + k * 32);   // Lmax >= 1
+    for (int k = 0; k < 7; ++k) cp_async_jc(ring + k * 32, jc + k * 32);
+    cp_async_commit();
+    int rd = 0;   // float4 offset of column j's slot
 
     // boundary values of column 1 (strips > 0): issue the slot load now, validate the tag at use
     float nMM = 0.f, nDG = 0.f, nMI = 0.f, nGD = 0.f, nIM = 0.f;
@@ -290,14 +306,20 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
     for (int r = 0; r < R; ++r) Y[r] = __fadd_rn(HHG_NEG, qs[r * 7 + 5].x);   // MI(., 0) = -FLT_MAX
 
     for (int j = 1; j <= Lmax; ++j) {
-      // ---- current column operands (from the prefetch registers), prefetch the next column
-      const float4 tp[5] = {nx[0], nx[1], nx[2], nx[3], nx[4]};
-      const float t_m2m = nx[5].x, t_m2d = nx[5].y, t_d2m = nx[5].z, t_d2d = nx[5].w;
-      const float t_i2m = nx[6].x, t_i2i = nx[6].y, t_m2i = nx[6].z;
-      const uint32_t t_ss = __float_as_uint(nx[6].w);
+      // ---- current column operands from the ring, then the copy of the next column into the other slot.  That slot
+      // held column j-1, whose LDS results column j-1 has already consumed, so the copy cannot overwrite unread data
+      cp_async_wait_all();
+      const float4* cur = ring + rd;
+      const float4 tp[5] = {cur[0], cur[32], cur[64], cur[96], cur[128]};
+      const float4 tt0 = cur[160], tt1 = cur[192];
+      const float t_m2m = tt0.x, t_m2d = tt0.y, t_d2m = tt0.z, t_d2d = tt0.w;
+      const float t_i2m = tt1.x, t_i2i = tt1.y, t_m2i = tt1.z;
+      const uint32_t t_ss = __float_as_uint(tt1.w);
+      rd ^= kJcSlot;
       jc += 224;
 #pragma unroll
-      for (int k = 0; k < 7; ++k) nx[k] = ld_jc(jc + k * 32);
+      for (int k = 0; k < 7; ++k) cp_async_jc(ring + rd + k * 32, jc + k * 32);
+      cp_async_commit();
 
       // ---- boundary row i0 at column j: slot prefetched during column j-1; wait until the producer strip's
       // tag is there, then prefetch column j+1
@@ -328,7 +350,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
       const float bcmp = (j <= Lt) ? best : INFINITY;   // padded columns never become the maximum
       float bc = bcmp;
 
-      // (t_ss & P.zero) is 0; it only keeps the 4th register of the prefetch LDG.128 live (see ld_slot)
+      // (t_ss & P.zero) is 0; it only keeps the 4th register of the operand LDS.128 live (see ld_slot)
       uint32_t word = SS ? 0u : (t_ss & P.zero);
 #pragma unroll
       for (int r = 0; r < R; ++r) {
@@ -440,6 +462,8 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
     const size_t o = ((size_t)P.job_ss_off[job] + s) * 32 + lane;
     P.strip_score[o] = best;
     P.strip_ij[o] = (bi << 16) | bj;
+    // the copy of column Lmax+1 (slack, never read) must land before the next item's first copy targets the ring
+    cp_async_wait_all();
     __syncwarp();   // all lanes done with the smem slice before the next TMA overwrites it
   }
 }

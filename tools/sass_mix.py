@@ -4,7 +4,7 @@ usage: python tools/sass_mix.py [--compile] [--lib PATH] [--all] [--filter SUBST
 
 For every k_viterbi<R,LOCAL,SS,CELLOFF> instantiation in the library it finds the column loop (see column_loop)
 and prints its static instructions per row visit (one row of one column for the 32 lanes of a warp) by opcode, the
-MOVs per column, registers, the size of the running-maximum rare path inside the loop and, with --compile, the
+MOVs, LDS (query rows and operand ring) and LDGSTS (cp.async into the ring) per column, registers, the size of the running-maximum rare path inside the loop and, with --compile, the
 spill bytes ptxas reports.  --compile builds the library with the flags of build.py into a
 temporary directory; otherwise --lib (default hh-suite_b200/libhhg.so) is read.
 """
@@ -138,7 +138,7 @@ def main() -> None:
             if t and a < int(t.group(1), 16) <= loop[-1][0]:
                 cold = max(cold, sum(a < x < int(t.group(1), 16) for x, _, _ in loop))
         print(f"{n}: {len(loop)} instructions per column = {len(loop) / R:.1f} per row visit; "
-              f"MOV {mix['MOV']} per column; {reg} registers, stack {stack} B"
+              f"MOV {mix['MOV']}, LDS {mix['LDS']}, LDGSTS {mix['LDGSTS']} per column; {reg} registers, stack {stack} B"
               + (f", spill stores {sp[0]} B / loads {sp[1]} B" if sp else "")
               + f"; widest skipped block {cold} ({(len(loop) - cold) / R:.1f} per row visit without it)")
         print("   " + "  ".join(f"{op} {c / R:.2f}" for op, c in mix.most_common()))
