@@ -437,17 +437,21 @@ def mac_debug_posterior(ctx, request, Lt):
     return out
 
 
-def query_from_hhm(ctx: "Context", record: bytes, R, params: "PrepParams | None" = None):
-    """hhg_query_from_hhm: PrepareQueryHMM (nocontxt) of one HHM record -> dict(L, p, tr, ss, pav, neff)."""
-    L, has_ss = hhm_scan(record)
+def _query_from(L: int, has_ss: bool, fn, *args):
+    """Shared body of query_from_hhm / query_from_a3m: fn(*args, L_cap, L_out, p, tr, ss, pav, neff) fills the arrays."""
     p = np.zeros((L + 2, 20), np.float32); tr = np.zeros((L + 1, 7), np.float32)
     ss = np.zeros(L + 2, np.uint8); pav = np.zeros(20, np.float32)
     neff = np.zeros(1, np.float32); Lo = np.zeros(1, np.int32)
+    _ck(fn(*args, L, _p(Lo, c_i32p), _p(p, c_f32p), _p(tr, c_f32p), _p(ss, c_u8p), _p(pav, c_f32p), _p(neff, c_f32p)))
+    return dict(L=L, p=p, tr=tr, ss=ss, pav=pav, neff=float(neff[0]), has_ss=has_ss)
+
+
+def query_from_hhm(ctx: "Context", record: bytes, R, params: "PrepParams | None" = None):
+    """hhg_query_from_hhm: PrepareQueryHMM (nocontxt) of one HHM record -> dict(L, p, tr, ss, pav, neff)."""
+    L, has_ss = hhm_scan(record)
     R = np.ascontiguousarray(R, np.float32)
     pp = params or PrepParams.defaults()
-    _ck(ctx.L.hhg_query_from_hhm(ctx.h, record, len(record), C.byref(pp), _p(R, c_f32p), L, _p(Lo, c_i32p), _p(p, c_f32p),
-                                 _p(tr, c_f32p), _p(ss, c_u8p), _p(pav, c_f32p), _p(neff, c_f32p)))
-    return dict(L=L, p=p, tr=tr, ss=ss, pav=pav, neff=float(neff[0]), has_ss=has_ss)
+    return _query_from(L, has_ss, ctx.L.hhg_query_from_hhm, ctx.h, record, len(record), C.byref(pp), _p(R, c_f32p))
 
 
 def a3m_scan(record: bytes, mp: "MsaParams | None" = None):
@@ -458,67 +462,71 @@ def a3m_scan(record: bytes, mp: "MsaParams | None" = None):
     return int(L[0]), int(N[0]), bool(ss[0])
 
 
-def a3m_parse(record: bytes, mp: "MsaParams | None" = None):
-    """hhg_a3m_parse (host only): what Alignment::Read + Compress + the first steps of Filter2 hold for one record."""
+def _msa_scan(record: bytes, seqs: "SeqDb | None", mp: "MsaParams"):
+    """(match columns, sequences) of an A3M record, or of a compressed one when seqs is given; host only."""
+    if seqs is None:
+        return a3m_scan(record, mp)[:2]
+    Lh = np.zeros(1, np.int32); Nh = np.zeros(1, np.int32)
+    _ck(load().hhg_ca3m_scan(record, len(record), C.byref(seqs), C.byref(mp), _p(Lh, c_i32p), _p(Nh, c_i32p)))
+    return int(Lh[0]), int(Nh[0])
+
+
+def _msa_parse(record: bytes, seqs: "SeqDb | None", mp: "MsaParams | None"):
+    """Shared body of a3m_parse / ca3m_parse (seqs given: compressed record)."""
     mp = mp or MsaParams.defaults()
-    L, N, _ = a3m_scan(record, mp)
+    L, N = _msa_scan(record, seqs, mp)
     dims = np.zeros(6, np.int32)
     X = np.zeros((N, L + 2), np.uint8); I = np.zeros((N, L + 2), np.uint16); keep = np.zeros(N, np.int8)
     nres = np.zeros(N, np.int32); ksort = np.zeros(N, np.int32)
-    _ck(load().hhg_a3m_parse(record, len(record), C.byref(mp), L, N, _p(dims, c_i32p), _p(X, c_u8p), I.ctypes.data,
-                             keep.ctypes.data, _p(nres, c_i32p), _p(ksort, c_i32p)))
+    out = (L, N, _p(dims, c_i32p), _p(X, c_u8p), I.ctypes.data, keep.ctypes.data, _p(nres, c_i32p), _p(ksort, c_i32p))
+    if seqs is None:
+        _ck(load().hhg_a3m_parse(record, len(record), C.byref(mp), *out))
+    else:
+        _ck(load().hhg_ca3m_parse(record, len(record), C.byref(seqs), C.byref(mp), *out))
     return dict(L=L, N_in=N, kfirst=int(dims[3]), kss_pred=int(dims[4]), kss_conf=int(dims[5]), X=X, I=I, keep=keep,
                 nres=nres, ksort=ksort)
 
 
+def a3m_parse(record: bytes, mp: "MsaParams | None" = None):
+    """hhg_a3m_parse (host only): what Alignment::Read + Compress + the first steps of Filter2 hold for one record."""
+    return _msa_parse(record, None, mp)
+
+
 def ca3m_parse(record: bytes, seqs: "SeqDb", mp: "MsaParams | None" = None):
     """hhg_ca3m_parse (host only): a compressed-alignment record as Alignment::ReadCompressed + Compress hold it."""
+    d = _msa_parse(record, seqs, mp)
+    del d["kss_pred"], d["kss_conf"]
+    return d
+
+
+def _to_hmm(ctx: "Context", record: bytes, seqs: "SeqDb | None", pb, S, mp: "MsaParams | None"):
+    """Shared body of msa_to_hmm / ca3m_to_hmm (seqs given: compressed record, whose ss row stays zero)."""
     mp = mp or MsaParams.defaults()
-    Lh = np.zeros(1, np.int32); Nh = np.zeros(1, np.int32)
-    _ck(load().hhg_ca3m_scan(record, len(record), C.byref(seqs), C.byref(mp), _p(Lh, c_i32p), _p(Nh, c_i32p)))
-    L, N = int(Lh[0]), int(Nh[0])
-    dims = np.zeros(6, np.int32)
-    X = np.zeros((N, L + 2), np.uint8); I = np.zeros((N, L + 2), np.uint16); keep = np.zeros(N, np.int8)
-    nres = np.zeros(N, np.int32); ksort = np.zeros(N, np.int32)
-    _ck(load().hhg_ca3m_parse(record, len(record), C.byref(seqs), C.byref(mp), L, N, _p(dims, c_i32p), _p(X, c_u8p),
-                              I.ctypes.data, keep.ctypes.data, _p(nres, c_i32p), _p(ksort, c_i32p)))
-    return dict(L=L, N_in=N, kfirst=int(dims[3]), X=X, I=I, keep=keep, nres=nres, ksort=ksort)
-
-
-def ca3m_to_hmm(ctx: "Context", record: bytes, seqs: "SeqDb", pb, S=None, mp: "MsaParams | None" = None):
-    """hhg_ca3m_to_hmm: one compressed-alignment record -> the raw HMM (see msa_to_hmm)."""
-    mp = mp or MsaParams.defaults()
-    Lh = np.zeros(1, np.int32); Nh = np.zeros(1, np.int32)
-    _ck(load().hhg_ca3m_scan(record, len(record), C.byref(seqs), C.byref(mp), _p(Lh, c_i32p), _p(Nh, c_i32p)))
-    L, N = int(Lh[0]), int(Nh[0])
-    dims = np.zeros(6, np.int32)
-    keep = np.zeros(N, np.int8); wg = np.zeros(N, np.float32)
-    f = np.zeros((L + 2, 20), np.float32); tr = np.zeros((L + 1, 7), np.float32); neff = np.zeros((3, L + 1), np.float32)
-    nh = np.zeros(1, np.float32)
-    pb = np.ascontiguousarray(pb, np.float32)
-    Sm = None if S is None else np.ascontiguousarray(S, np.float32)
-    _ck(ctx.L.hhg_ca3m_to_hmm(ctx.h, record, len(record), C.byref(seqs), C.byref(mp), _p(Sm, c_f32p), _p(pb, c_f32p), L, N,
-                              _p(dims, c_i32p), keep.ctypes.data, _p(wg, c_f32p), _p(f, c_f32p), _p(tr, c_f32p),
-                              _p(neff, c_f32p), _p(nh, c_f32p)))
-    return dict(L=L, N_in=N, N_filtered=int(dims[2]), kfirst=int(dims[3]), keep=keep, wg=wg, f=f, tr=tr, neff_m=neff[0],
-                neff_i=neff[1], neff_d=neff[2], neff_hmm=float(nh[0]), ss=np.zeros(L + 2, np.uint8))
-
-
-def msa_to_hmm(ctx: "Context", record: bytes, pb, S=None, mp: "MsaParams | None" = None):
-    """hhg_msa_to_hmm: one A3M record -> the HMM Alignment::FrequenciesAndTransitions computes (no pseudocounts)."""
-    mp = mp or MsaParams.defaults()
-    L, N, _ = a3m_scan(record, mp)
+    L, N = _msa_scan(record, seqs, mp)
     dims = np.zeros(6, np.int32)
     keep = np.zeros(N, np.int8); wg = np.zeros(N, np.float32)
     f = np.zeros((L + 2, 20), np.float32); tr = np.zeros((L + 1, 7), np.float32); neff = np.zeros((3, L + 1), np.float32)
     nh = np.zeros(1, np.float32); ss = np.zeros(L + 2, np.uint8)
     pb = np.ascontiguousarray(pb, np.float32)
     Sm = None if S is None else np.ascontiguousarray(S, np.float32)
-    _ck(ctx.L.hhg_msa_to_hmm(ctx.h, record, len(record), C.byref(mp), _p(Sm, c_f32p), _p(pb, c_f32p), L, N,
-                             _p(dims, c_i32p), keep.ctypes.data, _p(wg, c_f32p), _p(f, c_f32p), _p(tr, c_f32p),
-                             _p(neff, c_f32p), _p(nh, c_f32p), _p(ss, c_u8p)))
+    out = (_p(Sm, c_f32p), _p(pb, c_f32p), L, N, _p(dims, c_i32p), keep.ctypes.data, _p(wg, c_f32p), _p(f, c_f32p),
+           _p(tr, c_f32p), _p(neff, c_f32p), _p(nh, c_f32p))
+    if seqs is None:
+        _ck(ctx.L.hhg_msa_to_hmm(ctx.h, record, len(record), C.byref(mp), *out, _p(ss, c_u8p)))
+    else:
+        _ck(ctx.L.hhg_ca3m_to_hmm(ctx.h, record, len(record), C.byref(seqs), C.byref(mp), *out))
     return dict(L=L, N_in=N, N_filtered=int(dims[2]), kfirst=int(dims[3]), keep=keep, wg=wg, f=f, tr=tr, neff_m=neff[0],
                 neff_i=neff[1], neff_d=neff[2], neff_hmm=float(nh[0]), ss=ss)
+
+
+def ca3m_to_hmm(ctx: "Context", record: bytes, seqs: "SeqDb", pb, S=None, mp: "MsaParams | None" = None):
+    """hhg_ca3m_to_hmm: one compressed-alignment record -> the raw HMM (see msa_to_hmm)."""
+    return _to_hmm(ctx, record, seqs, pb, S, mp)
+
+
+def msa_to_hmm(ctx: "Context", record: bytes, pb, S=None, mp: "MsaParams | None" = None):
+    """hhg_msa_to_hmm: one A3M record -> the HMM Alignment::FrequenciesAndTransitions computes (no pseudocounts)."""
+    return _to_hmm(ctx, record, None, pb, S, mp)
 
 
 def query_from_a3m(ctx: "Context", record: bytes, R, pb, S=None, params: "PrepParams | None" = None,
@@ -526,16 +534,11 @@ def query_from_a3m(ctx: "Context", record: bytes, R, pb, S=None, params: "PrepPa
     """hhg_query_from_a3m: query alignment -> HMM -> PrepareQueryHMM (nocontxt) -> dict(L, p, tr, ss, pav, neff)."""
     mp = mp or MsaParams.defaults()
     L, _, has_ss = a3m_scan(record, mp)
-    p = np.zeros((L + 2, 20), np.float32); tr = np.zeros((L + 1, 7), np.float32)
-    ss = np.zeros(L + 2, np.uint8); pav = np.zeros(20, np.float32)
-    neff = np.zeros(1, np.float32); Lo = np.zeros(1, np.int32)
     R = np.ascontiguousarray(R, np.float32); pb = np.ascontiguousarray(pb, np.float32)
     Sm = None if S is None else np.ascontiguousarray(S, np.float32)
     pp = params or PrepParams.defaults()
-    _ck(ctx.L.hhg_query_from_a3m(ctx.h, record, len(record), C.byref(mp), _p(Sm, c_f32p), _p(pb, c_f32p), C.byref(pp),
-                                 _p(R, c_f32p), L, _p(Lo, c_i32p), _p(p, c_f32p), _p(tr, c_f32p), _p(ss, c_u8p),
-                                 _p(pav, c_f32p), _p(neff, c_f32p)))
-    return dict(L=L, p=p, tr=tr, ss=ss, pav=pav, neff=float(neff[0]), has_ss=has_ss)
+    return _query_from(L, has_ss, ctx.L.hhg_query_from_a3m, ctx.h, record, len(record), C.byref(mp), _p(Sm, c_f32p),
+                       _p(pb, c_f32p), C.byref(pp), _p(R, c_f32p))
 
 
 def cs219_parse(text: bytes, n_cap: int = 256):
@@ -601,21 +604,10 @@ class TargetDB:
         """Build the shard from HHM text records (`_hhm.ffdata` bytes + the offset/length columns of its
         `.ffindex`): getTemplateHMM + the query-independent part of PrepareTemplateHMM, once per database.
         R: the 20x20 pseudocount matrix (R[a][b], SetSubstitutionMatrix).  Call apply_null_model per query."""
-        off = np.ascontiguousarray(offsets, np.int64); ln = np.ascontiguousarray(lengths, np.int64)
-        n = len(off)
-        if n == 0 or len(ln) != n or off.min() < 0 or int((off + ln).max()) > len(data):
-            raise ValueError("offsets/lengths do not fit the data buffer")
         R = np.ascontiguousarray(R, np.float32)
         assert R.shape == (20, 20)
         pp = params or PrepParams.defaults()
-        h = C.c_void_p()
-        buf = np.frombuffer(data, np.uint8)        # bytes or a (read-only) mmap of the ffdata file
-        _ck(ctx.L.hhg_db_create_hhm(ctx.h, n, buf.ctypes.data_as(C.c_char_p), _p(off, c_i64p), _p(ln, c_i64p),
-                                    C.byref(pp), _p(R, c_f32p), C.byref(h)))
-        self = cls._wrap(ctx, h, n)
-        self.Lh = np.zeros(n, np.int32)
-        _ck(ctx.L.hhg_db_lengths(h, _p(self.Lh, c_i32p)))
-        return self
+        return cls._from_records(ctx, data, offsets, lengths, ctx.L.hhg_db_create_hhm, C.byref(pp), _p(R, c_f32p))
 
     @classmethod
     def from_a3m(cls, ctx, data: bytes, offsets, lengths, R, pb, S=None, params: "PrepParams | None" = None,
@@ -623,40 +615,36 @@ class TargetDB:
         """Build the shard from A3M alignments (`_a3m.ffdata` bytes + offset/length columns): the alignment branch of
         getTemplateHMM (Read, Compress, Filter, FrequenciesAndTransitions) + the query-independent part of
         PrepareTemplateHMM, once per database.  pb: background frequencies, S: substitution matrix in bits (qsc only)."""
-        off = np.ascontiguousarray(offsets, np.int64); ln = np.ascontiguousarray(lengths, np.int64)
-        n = len(off)
-        if n == 0 or len(ln) != n or off.min() < 0 or int((off + ln).max()) > len(data):
-            raise ValueError("offsets/lengths do not fit the data buffer")
-        R = np.ascontiguousarray(R, np.float32); pb = np.ascontiguousarray(pb, np.float32)
-        Sm = None if S is None else np.ascontiguousarray(S, np.float32)
-        pp = params or PrepParams.defaults()
-        mp = mp or MsaParams.defaults()
-        h = C.c_void_p()
-        buf = np.frombuffer(data, np.uint8)
-        _ck(ctx.L.hhg_db_create_a3m(ctx.h, n, buf.ctypes.data_as(C.c_char_p), _p(off, c_i64p), _p(ln, c_i64p),
-                                    C.byref(mp), _p(Sm, c_f32p), _p(pb, c_f32p), C.byref(pp), _p(R, c_f32p), C.byref(h)))
-        self = cls._wrap(ctx, h, n)
-        self.Lh = np.zeros(n, np.int32)
-        _ck(ctx.L.hhg_db_lengths(h, _p(self.Lh, c_i32p)))
-        return self
+        return cls._from_msa(ctx, data, offsets, lengths, None, R, pb, S, params, mp)
 
     @classmethod
     def from_ca3m(cls, ctx, data: bytes, offsets, lengths, seqs: "SeqDb", R, pb, S=None, params: "PrepParams | None" = None,
                   mp: "MsaParams | None" = None):
         """Build the shard from a compressed alignment database (`_ca3m.ffdata` + `_sequence.ffdata`, see SeqDb)."""
-        off = np.ascontiguousarray(offsets, np.int64); ln = np.ascontiguousarray(lengths, np.int64)
-        n = len(off)
-        if n == 0 or len(ln) != n or off.min() < 0 or int((off + ln).max()) > len(data):
-            raise ValueError("offsets/lengths do not fit the data buffer")
+        return cls._from_msa(ctx, data, offsets, lengths, seqs, R, pb, S, params, mp)
+
+    @classmethod
+    def _from_msa(cls, ctx, data: bytes, offsets, lengths, seqs, R, pb, S, params, mp):
+        """Shared body of from_a3m / from_ca3m (seqs given: compressed records)."""
         R = np.ascontiguousarray(R, np.float32); pb = np.ascontiguousarray(pb, np.float32)
         Sm = None if S is None else np.ascontiguousarray(S, np.float32)
         pp = params or PrepParams.defaults()
         mp = mp or MsaParams.defaults()
+        args = (C.byref(mp), _p(Sm, c_f32p), _p(pb, c_f32p), C.byref(pp), _p(R, c_f32p))
+        if seqs is None:
+            return cls._from_records(ctx, data, offsets, lengths, ctx.L.hhg_db_create_a3m, *args)
+        return cls._from_records(ctx, data, offsets, lengths, ctx.L.hhg_db_create_ca3m, C.byref(seqs), *args)
+
+    @classmethod
+    def _from_records(cls, ctx, data: bytes, offsets, lengths, create, *args):
+        """Shared body of the text-record loaders: create(ctx, n, data, offsets, lengths, *args, out) builds the shard."""
+        off = np.ascontiguousarray(offsets, np.int64); ln = np.ascontiguousarray(lengths, np.int64)
+        n = len(off)
+        if n == 0 or len(ln) != n or off.min() < 0 or int((off + ln).max()) > len(data):
+            raise ValueError("offsets/lengths do not fit the data buffer")
         h = C.c_void_p()
-        buf = np.frombuffer(data, np.uint8)
-        _ck(ctx.L.hhg_db_create_ca3m(ctx.h, n, buf.ctypes.data_as(C.c_char_p), _p(off, c_i64p), _p(ln, c_i64p),
-                                     C.byref(seqs), C.byref(mp), _p(Sm, c_f32p), _p(pb, c_f32p), C.byref(pp),
-                                     _p(R, c_f32p), C.byref(h)))
+        buf = np.frombuffer(data, np.uint8)        # bytes or a (read-only) mmap of the ffdata file
+        _ck(create(ctx.h, n, buf.ctypes.data_as(C.c_char_p), _p(off, c_i64p), _p(ln, c_i64p), *args, C.byref(h)))
         self = cls._wrap(ctx, h, n)
         self.Lh = np.zeros(n, np.int32)
         _ck(ctx.L.hhg_db_lengths(h, _p(self.Lh, c_i32p)))
