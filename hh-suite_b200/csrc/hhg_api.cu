@@ -220,11 +220,9 @@ struct hhg_plan {
   double cells = 0, padded_cells = 0, alg_bytes = 0;
   std::vector<int> ids;          // request -> target id
   std::vector<int> order;        // sorted position -> request index
-  std::vector<int> req_job, req_lane;   // per request
-  std::vector<int> job_Lmax, job_query, job_nstrips, job_Lq, job_qrow0;
-  std::vector<long long> job_ss_off;
+  std::vector<JobDesc> jobs;     // [njobs]
+  std::vector<ReqDesc> reqs;     // [n] in request order
   std::vector<int2> items;
-  std::vector<long long> job_bt_off, job_bnd_off, job_co_off, job_jc_off, path_off;
   long long jc_total = 0;                 // float4 in the job-interleaved operand stream
   unsigned long long jc_version = 0;      // db->cols_version the stream was built from (0 = never)
   int nm_mode = -1;                       // >= 0: columnscore of the null model fused into the stream (raw shard)
@@ -233,12 +231,11 @@ struct hhg_plan {
   std::vector<Wave> waves;
   long long path_total = 0;
   // device
-  DevBuf<int> d_job_target, d_job_Lmax, d_req_job, d_req_lane, d_req_Lt, d_req_Lq, d_req_target;
-  DevBuf<int> d_job_query, d_job_nstrips, d_job_Lq, d_job_qrow0;
-  DevBuf<long long> d_job_ss_off;
+  DevBuf<JobDesc> d_jobs;
+  DevBuf<ReqDesc> d_reqs;
+  DevBuf<int> d_job_target;
   DevBuf<int2> d_items;
   DevBuf<float> d_S;
-  DevBuf<long long> d_job_bt_off, d_job_bnd_off, d_job_co_off, d_job_jc_off, d_path_off;
   DevBuf<float4> d_jcols;
   DevBuf<uint32_t> d_bt, d_co;
   DevBuf<BndSlot> d_bnd;
@@ -1497,37 +1494,24 @@ static int plan_build(hhg_ctx* ctx, hhg_plan* pl, const hhg_db* db, int n, const
     return db->L[pl->ids[a]] > db->L[pl->ids[b]];
   });
   // jobs: runs of up to 32 consecutive sorted requests of the same query
-  std::vector<int> job_first, job_cnt;
-  for (int k = 0; k < n;) {
-    const int q = pl->req_query[pl->order[k]];
-    int e = k;
-    while (e < n && e - k < 32 && pl->req_query[pl->order[e]] == q) ++e;
-    job_first.push_back(k); job_cnt.push_back(e - k);
-    k = e;
-  }
-  pl->njobs = (int)job_first.size();
-  pl->req_job.resize(n); pl->req_lane.resize(n);
-  pl->job_Lmax.resize(pl->njobs); pl->job_query.resize(pl->njobs); pl->job_nstrips.resize(pl->njobs);
-  pl->job_Lq.resize(pl->njobs); pl->job_qrow0.resize(pl->njobs); pl->job_ss_off.resize(pl->njobs);
-  pl->job_bt_off.resize(pl->njobs); pl->job_bnd_off.resize(pl->njobs); pl->job_co_off.resize(pl->njobs);
-  pl->job_jc_off.resize(pl->njobs);
+  pl->jobs.clear();
+  pl->reqs.assign(n, ReqDesc{});
   pl->jc_version = 0;
-  std::vector<int> job_target((size_t)pl->njobs * 32);
-  std::vector<int> req_Lt(n), req_Lq(n);
+  std::vector<int> job_target;
   long long bnd = 0, co = 0, jc = 0, ss = 0;
   size_t wave_bt = 0, max_wave_words = 0;   // words in the current wave
   Wave w;
-  for (int jb = 0; jb < pl->njobs; ++jb) {
-    const int first = job_first[jb], cnt = job_cnt[jb];
+  for (int first = 0; first < n;) {
+    const int jb = (int)pl->jobs.size();
     const int q = pl->req_query[pl->order[first]];
+    int cnt = 0;
+    while (first + cnt < n && cnt < 32 && pl->req_query[pl->order[first + cnt]] == q) ++cnt;
     const int Lmax = db->L[pl->ids[pl->order[first]]];
     const int ns = (ctx->q_L[q] + R - 1) / R;
-    pl->job_Lmax[jb] = Lmax; pl->job_query[jb] = q; pl->job_nstrips[jb] = ns;
-    pl->job_Lq[jb] = ctx->q_L[q]; pl->job_qrow0[jb] = ctx->q_row0[q];
     for (int l = 0; l < 32; ++l) {
       const int rq = pl->order[first + std::min(l, cnt - 1)];   // padded lanes repeat the last target
-      job_target[(size_t)jb * 32 + l] = pl->ids[rq];
-      if (l < cnt) { pl->req_job[rq] = jb; pl->req_lane[rq] = l; }
+      job_target.push_back(pl->ids[rq]);
+      if (l < cnt) { pl->reqs[rq].job = jb; pl->reqs[rq].lane = l; }
     }
     const size_t words = (size_t)(ns * R / 4) * (Lmax + 1) * 32;
     if (wave_bt > 0 && (wave_bt + words) * 4 > ctx->max_bt_bytes) {
@@ -1537,18 +1521,19 @@ static int plan_build(hhg_ctx* ctx, hhg_plan* pl, const hhg_db* db, int n, const
       w.job_begin = jb;
       wave_bt = 0;
     }
-    pl->job_bt_off[jb] = (long long)wave_bt;
+    JobDesc d{};
+    d.ss_off = ss; d.bt_off = (long long)wave_bt; d.bnd_off = bnd; d.co_off = co; d.jc_off = jc;
+    d.Lmax = Lmax; d.query = q; d.nstrips = ns; d.Lq = ctx->q_L[q]; d.qrow0 = ctx->q_row0[q];
+    pl->jobs.push_back(d);
     wave_bt += words;
-    pl->job_bnd_off[jb] = bnd;
     bnd += (long long)(Lmax + 1) * 32;
-    pl->job_co_off[jb] = co;
-    pl->job_jc_off[jb] = jc;
-    pl->job_ss_off[jb] = ss;
     jc += (long long)Lmax * 224;
     co += (long long)ns * (Lmax + 1) * 32;
     ss += ns;
     pl->padded_cells += (double)ns * R * (double)Lmax * 32.0;
+    first += cnt;
   }
+  pl->njobs = (int)pl->jobs.size();
   w.job_end = pl->njobs;
   pl->waves.push_back(w);
   max_wave_words = std::max(max_wave_words, wave_bt);
@@ -1562,24 +1547,24 @@ static int plan_build(hhg_ctx* ctx, hhg_plan* pl, const hhg_db* db, int n, const
     for (int g0 = wv.job_begin; g0 < wv.job_end; g0 += ctx->group_jobs) {
       const int g1 = std::min(g0 + ctx->group_jobs, wv.job_end);
       int maxns = 0;
-      for (int jb = g0; jb < g1; ++jb) maxns = std::max(maxns, pl->job_nstrips[jb]);
+      for (int jb = g0; jb < g1; ++jb) maxns = std::max(maxns, pl->jobs[jb].nstrips);
       for (int sidx = 0; sidx < maxns; ++sidx)
         for (int jb = g0; jb < g1; ++jb)
-          if (sidx < pl->job_nstrips[jb]) pl->items.push_back(make_int2(jb - wv.job_begin, sidx));
+          if (sidx < pl->jobs[jb].nstrips) pl->items.push_back(make_int2(jb - wv.job_begin, sidx));
     }
     wv.item_end = (long long)pl->items.size();
   }
-  pl->path_off.resize(n);
   long long po = 0;
   double cols_sum = 0;
   for (int k = 0; k < n; ++k) {
-    const int Lt = db->L[pl->ids[k]];
-    const int Lqk = ctx->q_L[pl->req_query[k]];
-    req_Lt[k] = Lt; req_Lq[k] = Lqk;
-    pl->path_off[k] = po;
-    po += Lqk + Lt + 2;
-    pl->cells += (double)Lqk * Lt;
-    cols_sum += Lt;
+    ReqDesc& r = pl->reqs[k];
+    r.target = pl->ids[k];
+    r.Lt = db->L[r.target];
+    r.Lq = ctx->q_L[pl->req_query[k]];
+    r.path_off = po;
+    po += r.Lq + r.Lt + 2;
+    pl->cells += (double)r.Lq * r.Lt;
+    cols_sum += r.Lt;
   }
   if (po > 0x7fffffffLL) return fail(HHG_EINVAL, "plan too large: %lld path bytes (> 2^31-1); split the request", po);
   pl->path_total = po;
@@ -1588,16 +1573,12 @@ static int plan_build(hhg_ctx* ctx, hhg_plan* pl, const hhg_db* db, int n, const
 
   cudaError_t e = cudaSuccess;
   auto A = [&](cudaError_t r) { if (e == cudaSuccess) e = r; };
-  A(pl->d_job_target.ensure(job_target.size())); A(pl->d_job_Lmax.ensure(pl->njobs));
-  A(pl->d_job_bt_off.ensure(pl->njobs)); A(pl->d_job_bnd_off.ensure(pl->njobs)); A(pl->d_job_co_off.ensure(pl->njobs));
+  A(pl->d_jobs.ensure(pl->njobs)); A(pl->d_reqs.ensure(n));
+  A(pl->d_job_target.ensure(job_target.size())); A(pl->d_items.ensure(pl->items.size()));
   // one column (224 float4) and one slot column (32 slots) of slack: k_viterbi prefetches column j+1 unconditionally,
   // so at the last job's last column it reads one column past the operand stream and the slots (never used)
-  A(pl->d_job_jc_off.ensure(pl->njobs)); A(pl->d_jcols.ensure((size_t)jc + 224));
-  A(pl->d_job_query.ensure(pl->njobs)); A(pl->d_job_nstrips.ensure(pl->njobs)); A(pl->d_job_Lq.ensure(pl->njobs));
-  A(pl->d_job_qrow0.ensure(pl->njobs)); A(pl->d_job_ss_off.ensure(pl->njobs)); A(pl->d_items.ensure(pl->items.size()));
-  A(pl->d_req_job.ensure(n)); A(pl->d_req_lane.ensure(n)); A(pl->d_req_Lt.ensure(n)); A(pl->d_req_Lq.ensure(n));
-  A(pl->d_path_off.ensure(n));
-  A(pl->d_req_target.ensure(n)); A(pl->d_S.ensure((size_t)po));
+  A(pl->d_jcols.ensure((size_t)jc + 224));
+  A(pl->d_S.ensure((size_t)po));
   A(pl->d_bt.ensure(max_wave_words));
   { BndSlot* before = pl->d_bnd.p; A(pl->d_bnd.ensure((size_t)bnd + 32));
     // fresh slots must not carry a bit pattern that looks like a valid tag (epochs start at 1)
@@ -1611,24 +1592,10 @@ static int plan_build(hhg_ctx* ctx, hhg_plan* pl, const hhg_db* db, int n, const
 
   cudaStream_t st = ctx->stream;
   auto H2D = [&](void* d, const void* h, size_t bytes) { return cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st); };
+  CK(H2D(pl->d_jobs.p, pl->jobs.data(), pl->jobs.size() * sizeof(JobDesc)));
+  CK(H2D(pl->d_reqs.p, pl->reqs.data(), pl->reqs.size() * sizeof(ReqDesc)));
   CK(H2D(pl->d_job_target.p, job_target.data(), job_target.size() * 4));
-  CK(H2D(pl->d_job_Lmax.p, pl->job_Lmax.data(), (size_t)pl->njobs * 4));
-  CK(H2D(pl->d_job_bt_off.p, pl->job_bt_off.data(), (size_t)pl->njobs * 8));
-  CK(H2D(pl->d_job_bnd_off.p, pl->job_bnd_off.data(), (size_t)pl->njobs * 8));
-  CK(H2D(pl->d_job_co_off.p, pl->job_co_off.data(), (size_t)pl->njobs * 8));
-  CK(H2D(pl->d_job_jc_off.p, pl->job_jc_off.data(), (size_t)pl->njobs * 8));
-  CK(H2D(pl->d_job_query.p, pl->job_query.data(), (size_t)pl->njobs * 4));
-  CK(H2D(pl->d_job_nstrips.p, pl->job_nstrips.data(), (size_t)pl->njobs * 4));
-  CK(H2D(pl->d_job_Lq.p, pl->job_Lq.data(), (size_t)pl->njobs * 4));
-  CK(H2D(pl->d_job_qrow0.p, pl->job_qrow0.data(), (size_t)pl->njobs * 4));
-  CK(H2D(pl->d_job_ss_off.p, pl->job_ss_off.data(), (size_t)pl->njobs * 8));
   CK(H2D(pl->d_items.p, pl->items.data(), pl->items.size() * sizeof(int2)));
-  CK(H2D(pl->d_req_job.p, pl->req_job.data(), (size_t)n * 4));
-  CK(H2D(pl->d_req_lane.p, pl->req_lane.data(), (size_t)n * 4));
-  CK(H2D(pl->d_req_Lt.p, req_Lt.data(), (size_t)n * 4));
-  CK(H2D(pl->d_req_Lq.p, req_Lq.data(), (size_t)n * 4));
-  CK(H2D(pl->d_req_target.p, pl->ids.data(), (size_t)n * 4));
-  CK(H2D(pl->d_path_off.p, pl->path_off.data(), (size_t)n * 8));
   CK(cudaStreamSynchronize(st));
   return HHG_OK;
 }
@@ -1674,9 +1641,8 @@ static int set_exclusions(hhg_ctx* ctx, hhg_plan* pl, const int64_t* excl_off, c
     std::vector<int> sreq((size_t)total);
     for (int k = 0; k < pl->n; ++k) {
       if (excl_off[k + 1] < excl_off[k]) return fail(HHG_EINVAL, "excl_off is not monotonic at request %d", k);
-      const int Lt = pl->db->L[pl->ids[k]];
+      const int Lt = pl->reqs[k].Lt, Lqk = pl->reqs[k].Lq;
       for (long long s = excl_off[k]; s < excl_off[k + 1]; ++s) {
-        const int Lqk = pl->q_L[pl->req_query[k]];
         if (excl_i[s] < 1 || excl_i[s] > Lqk || excl_j[s] < 1 || excl_j[s] > Lt)
           return fail(HHG_EINVAL, "excluded step %lld of request %d is (%d,%d), outside 1..%d x 1..%d", s - excl_off[k], k,
                       excl_i[s], excl_j[s], Lqk, Lt);
@@ -1689,8 +1655,7 @@ static int set_exclusions(hhg_ctx* ctx, hhg_plan* pl, const int64_t* excl_off, c
     CK(cudaMemcpyAsync(pl->d_step_j.p, excl_j, (size_t)total * 4, cudaMemcpyHostToDevice, ctx->stream));
     const int threads = 128;
     k_celloff_raster<<<(unsigned)((total + threads - 1) / threads), threads, 0, ctx->stream>>>(
-        (int)total, pl->d_step_req.p, pl->d_step_i.p, pl->d_step_j.p, pl->d_req_job.p, pl->d_req_lane.p,
-        pl->d_req_Lt.p, pl->d_req_Lq.p, pl->d_job_Lmax.p, pl->d_job_co_off.p, pl->R, pl->d_co.p);
+        (int)total, pl->d_step_req.p, pl->d_step_i.p, pl->d_step_j.p, pl->d_reqs.p, pl->d_jobs.p, pl->R, pl->d_co.p);
     ctx->launches++;
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(ctx->stream));   // sreq is a host temporary
@@ -1701,8 +1666,7 @@ static int set_exclusions(hhg_ctx* ctx, hhg_plan* pl, const int64_t* excl_off, c
     if (rc != HHG_OK) return rc;
     const int* d = ctx->d_ex.p;
     k_celloff_regions<<<(unsigned)((co_words + 255) / 256), 256, 0, ctx->stream>>>(
-        (long long)co_words, pl->njobs, pl->d_job_co_off.p, pl->d_job_Lmax.p, pl->d_job_nstrips.p, pl->R, nq, d, d + nq,
-        nt, d + 2 * nq, d + 2 * nq + nt, pl->d_co.p);
+        (long long)co_words, pl->njobs, pl->d_jobs.p, pl->R, nq, d, d + nq, nt, d + 2 * nq, d + 2 * nq + nt, pl->d_co.p);
     ctx->launches++;
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(ctx->stream));
@@ -1779,11 +1743,11 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
     // (re)build the job-interleaved operand stream: once per plan, again after every hhg_db_apply_null_model (the
     // prepared emissions changed) and, with the fused null model, for every new query batch
     int maxL = 0;
-    for (int jb = 0; jb < pl->njobs; ++jb) maxL = std::max(maxL, pl->job_Lmax[jb]);
+    for (const JobDesc& jd : pl->jobs) maxL = std::max(maxL, jd.Lmax);
     dim3 grid((unsigned)pl->njobs, (unsigned)std::min(64, (maxL + 7) / 8), 1);
-    k_interleave_cols<<<grid, 256, 0, st>>>(pl->njobs, pl->d_job_target.p, pl->d_job_Lmax.p, pl->d_job_jc_off.p,
-                                            fused ? db->cols_raw.p : db->cols.p, db->dcol_off.p, db->dL.p, pl->d_jcols.p,
-                                            pl->nm_mode, pl->d_job_query.p, ctx->d_q_pav.p, db->pav.p, ctx->d_pb.p);
+    k_interleave_cols<<<grid, 256, 0, st>>>(pl->d_jobs.p, pl->d_job_target.p, fused ? db->cols_raw.p : db->cols.p,
+                                            db->dcol_off.p, db->dL.p, pl->d_jcols.p, pl->nm_mode, ctx->d_q_pav.p,
+                                            db->pav.p, ctx->d_pb.p);
     ctx->launches++;
     CK(cudaGetLastError());
     pl->jc_version = db->cols_version;
@@ -1795,22 +1759,16 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
     const int nj = w.job_end - w.job_begin;
     VitParams P{};
     P.qrec = ctx->qrec.p;
-    P.job_Lq = pl->d_job_Lq.p + w.job_begin; P.job_nstrips = pl->d_job_nstrips.p + w.job_begin;
-    P.job_qrow0 = pl->d_job_qrow0.p + w.job_begin; P.job_ss_off = pl->d_job_ss_off.p + w.job_begin;
+    P.jobs = pl->d_jobs.p + w.job_begin;
     P.items = pl->d_items.p + w.item_begin; P.n_items = (int)(w.item_end - w.item_begin);
     P.Lt = db->dL.p;
     P.jcols = pl->d_jcols.p;
-    P.job_jc_off = pl->d_job_jc_off.p + w.job_begin;
     P.njobs = nj;
     P.job_target = pl->d_job_target.p + (size_t)w.job_begin * 32;
-    P.job_Lmax = pl->d_job_Lmax.p + w.job_begin;
-    P.job_bt_off = pl->d_job_bt_off.p + w.job_begin;
-    P.job_bnd_off = pl->d_job_bnd_off.p + w.job_begin;
-    P.job_co_off = pl->d_job_co_off.p + w.job_begin;
     P.bt = pl->d_bt.p; P.bnd = pl->d_bnd.p;
     P.tag_base = ctx->epoch << 12;
     P.counter = pl->d_counter.p + wi;
-    P.strip_score = pl->d_strip_score.p;     // job_ss_off is absolute
+    P.strip_score = pl->d_strip_score.p;     // JobDesc::ss_off is absolute
     P.strip_ij = pl->d_strip_ij.p;
     P.celloff = pl->celloff ? pl->d_co.p : nullptr;
     P.S33 = ctx->has_S33 ? ctx->S33.p : nullptr;
@@ -1825,19 +1783,15 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
     else rc = launch_viterbi<16>(ctx, P, ctx->par.local != 0, ctx->par.use_ss != 0, pl->celloff, items);
     if (rc != HHG_OK) return rc;
     if (timed) CK(cudaEventRecord(ctx->ev[1], st));
-    // backtrace of this wave's requests.  Requests are addressed through the sorted order: the
-    // wave covers sorted positions [req_begin, req_end); req_job/req_lane are per original request.
+    // backtrace of this wave's requests: every request whose job lies in the wave (ReqDesc::job is absolute)
     BtParams B{};
     B.n_req = pl->n;   // filtered by job range inside: simpler to launch per wave over all requests
-    B.job_nstrips = pl->d_job_nstrips.p; B.job_ss_off = pl->d_job_ss_off.p; B.job_qrow0 = pl->d_job_qrow0.p;
-    B.nm_mode = pl->nm_mode; B.job_query = pl->d_job_query.p; B.q_pav = ctx->d_q_pav.p; B.t_pav = db->pav.p;
-    B.pb = ctx->d_pb.p;
-    B.req_job = pl->d_req_job.p; B.req_lane = pl->d_req_lane.p;
-    B.job_Lmax = pl->d_job_Lmax.p; B.job_bt_off = pl->d_job_bt_off.p;
+    B.jobs = pl->d_jobs.p; B.reqs = pl->d_reqs.p;
+    B.nm_mode = pl->nm_mode; B.q_pav = ctx->d_q_pav.p; B.t_pav = db->pav.p; B.pb = ctx->d_pb.p;
     B.bt = pl->d_bt.p; B.strip_score = pl->d_strip_score.p; B.strip_ij = pl->d_strip_ij.p;
-    B.path_off = pl->d_path_off.p; B.hits = pl->d_hits.p; B.paths = pl->d_paths.p;
+    B.hits = pl->d_hits.p; B.paths = pl->d_paths.p;
     B.job_begin = w.job_begin; B.job_end = w.job_end;
-    B.req_target = pl->d_req_target.p; B.qrec = ctx->qrec.p; B.cols = fused ? db->cols_raw.p : db->cols.p; B.col_off = db->dcol_off.p;
+    B.qrec = ctx->qrec.p; B.cols = fused ? db->cols_raw.p : db->cols.p; B.col_off = db->dcol_off.p;
     B.lg2 = ctx->lg2.p; B.diff = ctx->diff.p; B.S33 = ctx->has_S33 ? ctx->S33.p : nullptr; B.S = pl->d_S.p;
     B.corr = ctx->par.corr; B.ssw = ctx->par.ssw; B.use_ss = ctx->par.use_ss; B.ss_score_mode = (ctx->par.ssm == 2);
     const int threads = 128;
@@ -1891,7 +1845,7 @@ int hhg_plan_fetch(hhg_ctx* ctx, hhg_plan* pl, hhg_hit* hits, uint8_t* paths, si
     CK(cudaMemcpyAsync(pl->d_compact_off.p, pl->h_compact_off.data(), (size_t)pl->n * 8, cudaMemcpyHostToDevice, ctx->stream));
     const int threads = 128;
     k_gather_paths<<<(pl->n + threads - 1) / threads, threads, 0, ctx->stream>>>(
-        pl->n, pl->d_hits.p, pl->d_path_off.p, pl->d_compact_off.p, pl->d_paths.p, pl->d_paths_compact.p);
+        pl->n, pl->d_hits.p, pl->d_reqs.p, pl->d_compact_off.p, pl->d_paths.p, pl->d_paths_compact.p);
     ctx->launches++;
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(paths, pl->d_paths_compact.p, (size_t)tot, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1908,14 +1862,13 @@ int hhg_plan_debug_bt(hhg_ctx* ctx, hhg_plan* pl, int k, uint8_t* bt) {
   if (!ctx || !pl || !bt || k < 0 || k >= pl->n) return fail(HHG_EINVAL, "hhg_plan_debug_bt: bad argument");
   if (pl->waves.size() != 1) return fail(HHG_EINVAL, "debug_bt needs a single-wave plan");
   CK(cudaSetDevice(ctx->device));
-  const int job = pl->req_job[k], lane = pl->req_lane[k];
-  const int Lt = pl->db->L[pl->ids[k]];
-  const int Lqk = pl->q_L[pl->req_query[k]];
-  const int total = (Lqk + 1) * (Lt + 1);
+  const ReqDesc& rq = pl->reqs[k];
+  const JobDesc& jd = pl->jobs[rq.job];
+  const int total = (rq.Lq + 1) * (rq.Lt + 1);
   DevBuf<uint8_t> tmp;
   CK(tmp.alloc(total));
-  k_debug_bt<<<(total + 255) / 256, 256, 0, ctx->stream>>>(pl->d_bt.p, pl->job_bt_off[job], lane,
-                                                            pl->job_Lmax[job], Lqk, Lt, tmp.p);
+  k_debug_bt<<<(total + 255) / 256, 256, 0, ctx->stream>>>(pl->d_bt.p, jd.bt_off, rq.lane, jd.Lmax, rq.Lq, rq.Lt,
+                                                            tmp.p);
   ctx->launches++;
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(bt, tmp.p, total, cudaMemcpyDeviceToHost, ctx->stream));

@@ -93,13 +93,36 @@ __device__ __forceinline__ bool slot_ok(const uint32_t (&tag)[5], uint32_t want)
   return ((tag[0] ^ want) | (tag[1] ^ want) | (tag[2] ^ want) | (tag[3] ^ want) | (tag[4] ^ want)) == 0u;
 }
 
+// One 32-target warp job of a plan (plan_build): up to 32 length-sorted requests of one query, one per lane.
+struct JobDesc {
+  long long ss_off;   // offset (in 32-lane blocks) of the job's per-strip maxima (absolute over all waves)
+  long long bt_off;   // offset (in uint32 words) into bt, relative to the job's memory wave
+  long long bnd_off;  // offset (in slots) into bnd
+  long long co_off;   // offset (in uint32 words) of the job's cell-off words
+  long long jc_off;   // offset (in float4) of the job's operand stream
+  int Lmax;           // length of the job's longest (first) target
+  int query;          // index of the job's query in the query batch
+  int nstrips;        // ceil(Lq / R)
+  int Lq;             // length of the job's query
+  int qrow0;          // first row record of the job's query in qrec
+};
+static_assert(sizeof(JobDesc) == 64, "JobDesc: 5 x int64 + 5 x int32, tail padding only");
+
+// One request of a plan: one (query, target) alignment, traced by lane `lane` of job `job`.
+struct ReqDesc {
+  long long path_off;  // offset into the plan's path bytes and per-step scores (capacity Lq + Lt + 2)
+  int job;             // absolute job index
+  int lane;            // lane in the job
+  int target;          // target id in the shard
+  int Lt;              // target length
+  int Lq;              // query length
+};
+static_assert(sizeof(ReqDesc) == 32, "ReqDesc: 1 x int64 + 5 x int32, tail padding only");
+
 struct VitParams {
   // queries: a plan may hold several (query-batch mode, hhblits_omp semantics); every job belongs to one of them
   const float4* qrec;        // query row records (rows 1..Lq of every query, each block zero padded to a multiple of 48)
-  const int* job_Lq;         // [njobs] length of the job's query
-  const int* job_nstrips;    // [njobs] ceil(Lq / R)
-  const int* job_qrow0;      // [njobs] first row record of the job's query in qrec
-  const long long* job_ss_off;   // [njobs] offset (in 32-lane blocks) of the job's per-strip maxima
+  const JobDesc* jobs;       // [njobs] this wave's jobs (item job indices are relative to the wave)
   const int2* items;         // [n_items] work items (job, strip) in dispatch order (see plan_build)
   int n_items;
   // database shard
@@ -107,13 +130,9 @@ struct VitParams {
   // plan: the job-interleaved operand stream, [job][column 1..Lmax][k 0..6][lane] float4 (lanes shorter than
   // the job repeat their last column; the cells computed there are never used)
   const float4* jcols;
-  const long long* job_jc_off;   // [njobs] offset (in float4) of the job's stream
   // plan
   int njobs;
   const int* job_target;     // [njobs*32] target id (padded lanes repeat a valid id)
-  const int* job_Lmax;       // [njobs]
-  const long long* job_bt_off;   // [njobs] offset (in uint32 words) into bt
-  const long long* job_bnd_off;  // [njobs] offset (in slots) into bnd
   uint32_t* bt;              // packed backtrace words
   struct BndSlot* bnd;       // boundary hand-off slots [job][col][32 lanes], 40 B each (see BndSlot)
   uint32_t tag_base;         // run epoch << 12; slot tag = tag_base + strip + 1
@@ -121,7 +140,6 @@ struct VitParams {
   float* strip_score;        // [njobs*nstrips*32]
   int* strip_ij;             // [njobs*nstrips*32]  (i<<16 | j)
   const uint32_t* celloff;   // [sum over jobs nstrips*(Lmax+1)*32] bit r = row i0+1+r off, or null
-  const long long* job_co_off;
   const float* S33;          // [44*44] or null
   // scoring
   float egq, egt, shift, ssw;
@@ -245,31 +263,34 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
     // one job are dispatched G items apart (natural skew) while the group's targets stay L2-resident
     const int2 it = __ldg(P.items + item);
     const int job = it.x, s = it.y;
-    const int Lq = P.job_Lq[job];
-    const int nstrips = P.job_nstrips[job];
+    // job fields are read where they are used: a copy of the whole JobDesc would keep its offsets live across the
+    // column loop
+    const JobDesc* jd = P.jobs + job;
+    const int Lq = jd->Lq;
+    const int nstrips = jd->nstrips;
     const int i0 = s * R;
 
     // ---- stage this strip's query rows with one TMA bulk copy
     if (lane == 0) {
       mbar_expect_tx(bar, R * 112);
-      tma_bulk_g2s(qs, P.qrec + (size_t)(P.job_qrow0[job] + i0) * 7, R * 112, bar);
+      tma_bulk_g2s(qs, P.qrec + (size_t)(jd->qrow0 + i0) * 7, R * 112, bar);
     }
 
     const int t = P.job_target[job * 32 + lane];
     const int Lt = P.Lt[t];
-    const int Lmax = P.job_Lmax[job];
+    const int Lmax = jd->Lmax;
     // per-column pointers advance by constants: the operand stream by 7 x 32 float4, slots and backtrace words by 32.
     // The plan allocates one column of slack after the last job's stream and slots, so the copy of column j+1 into
     // the ring needs no clamp (what it reads after the job's last column is never used)
-    const float4* jc = P.jcols + P.job_jc_off[job] + lane;   // operand k of the prefetched column: jc[k*32]
+    const float4* jc = P.jcols + jd->jc_off + lane;   // operand k of the prefetched column: jc[k*32]
     const size_t bt_row_stride = (size_t)(Lmax + 1) * 32;   // words per 4-row group
-    uint32_t* btc = P.bt + P.job_bt_off[job] + lane + (size_t)(i0 >> 2) * bt_row_stride + 32;   // column j
-    BndSlot* bndc = P.bnd + P.job_bnd_off[job] + 32;          // the job's 32 slots of column j
+    uint32_t* btc = P.bt + jd->bt_off + lane + (size_t)(i0 >> 2) * bt_row_stride + 32;   // column j
+    BndSlot* bndc = P.bnd + jd->bnd_off + 32;          // the job's 32 slots of column j
     const uint32_t tag_in = P.tag_base + (uint32_t)s;        // written by strip s-1
     const uint32_t tag_out = P.tag_base + (uint32_t)s + 1u;  // what this strip writes
     const bool last_strip = (s == nstrips - 1);
     const uint32_t* co = nullptr;                            // column j
-    if (CELLOFF) co = P.celloff + P.job_co_off[job] + (size_t)s * (Lmax + 1) * 32 + lane + 32;
+    if (CELLOFF) co = P.celloff + jd->co_off + (size_t)s * (Lmax + 1) * 32 + lane + 32;
 
     // ---- state of the R rows at the previous column (column 0 initially), :161-173.
     // Every array element is read by its own row before the row overwrites it, so the state updates in place:
@@ -459,7 +480,11 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
       btc += 32;
       if (CELLOFF) co += 32;
     }
-    const size_t o = ((size_t)P.job_ss_off[job] + s) * 32 + lane;
+    // the job's address is formed again from the opaque index: reusing jd would keep that 64-bit pointer live across
+    // the column loop, and that loop measured 0.8 % slower at R = 16 (H100 80GB HBM3, 700 W power limit)
+    int jb = job;
+    asm("" : "+r"(jb));
+    const size_t o = ((size_t)P.jobs[jb].ss_off + s) * 32 + lane;
     P.strip_score[o] = best;
     P.strip_ij[o] = (bi << 16) | bj;
     // the copy of column Lmax+1 (slack, never read) must land before the next item's first copy targets the ring
@@ -501,29 +526,21 @@ struct HitRec {
 
 struct BtParams {
   int n_req;
-  const int* job_nstrips;    // [njobs]
-  const long long* job_ss_off;
-  const int* job_qrow0;      // [njobs] first row record of the job's query
+  const JobDesc* jobs;       // [njobs] all of the plan's jobs (absolute job index)
+  const ReqDesc* reqs;       // [n_req]
   // fused null model (query-batch plans over a raw shard): cols = emissions BEFORE the null model and the division
   // t.p[j][a] / pnul[a] is applied on the fly exactly like HMM::IncludeNullModelInHMM; nm_mode < 0: cols are prepared
   int nm_mode;
-  const int* job_query;      // [njobs]
   const float* q_pav;        // [nq*20]
   const float* t_pav;        // [n_targets*20]
   const float* pb;           // [20]
   int job_begin, job_end;    // only requests whose job lies in [job_begin, job_end) are traced
-  const int* req_job;        // [n_req]
-  const int* req_lane;       // [n_req]
-  const int* job_Lmax;
-  const long long* job_bt_off;
   const uint32_t* bt;
   const float* strip_score;
   const int* strip_ij;
-  const long long* path_off; // [n_req] offsets into paths
   HitRec* hits;
   uint8_t* paths;            // may be null
   // Hit.score (Viterbi::ScoreForBacktrace, src/hhviterbi.cpp:195-281)
-  const int* req_target;     // [n_req] target id in the shard
   const float4* qrec;        // query row records (p in the first 5 float4)
   const float4* cols;        // target column records
   const long long* col_off;
@@ -563,31 +580,31 @@ __device__ __forceinline__ uint32_t bt_byte(const uint32_t* btj, size_t row_stri
 __global__ void k_backtrace(const BtParams P) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= P.n_req) return;
-  const int job = P.req_job[k], lane = P.req_lane[k];
+  const ReqDesc rq = P.reqs[k];
+  const int job = rq.job, lane = rq.lane;
   if (job < P.job_begin || job >= P.job_end) return;
+  const JobDesc jd = P.jobs[job];
   float best = HHG_NEG;
   int ij = 0;
-  const int nstrips = P.job_nstrips[job];
-  for (int s = 0; s < nstrips; ++s) {
-    const size_t o = ((size_t)P.job_ss_off[job] + s) * 32 + lane;
+  for (int s = 0; s < jd.nstrips; ++s) {
+    const size_t o = ((size_t)jd.ss_off + s) * 32 + lane;
     const float v = P.strip_score[o];
     if (v > best) { best = v; ij = P.strip_ij[o]; }
   }
   const int i2 = ij >> 16, j2 = ij & 0xFFFF;
-  const int Lmax = P.job_Lmax[job];
-  const uint32_t* btj = P.bt + P.job_bt_off[job] + lane;
-  const size_t rs = (size_t)(Lmax + 1) * 32;
-  uint8_t* path = P.paths ? P.paths + P.path_off[k] : nullptr;
+  const uint32_t* btj = P.bt + jd.bt_off + lane;
+  const size_t rs = (size_t)(jd.Lmax + 1) * 32;
+  uint8_t* path = P.paths ? P.paths + rq.path_off : nullptr;
 
-  const float4* tcol = P.cols + (size_t)P.col_off[P.req_target[k]] * 7;
-  const float4* qrec = P.qrec + (size_t)P.job_qrow0[job] * 7;
+  const float4* tcol = P.cols + (size_t)P.col_off[rq.target] * 7;
+  const float4* qrec = P.qrec + (size_t)jd.qrow0 * 7;
   float pnv[20];
   const float* pn = nullptr;
   if (P.nm_mode >= 0) {
-    null_model_vec(P.nm_mode, P.q_pav + (size_t)P.job_query[job] * 20, P.t_pav + (size_t)P.req_target[k] * 20, P.pb, pnv);
+    null_model_vec(P.nm_mode, P.q_pav + (size_t)jd.query * 20, P.t_pav + (size_t)rq.target * 20, P.pb, pnv);
     pn = pnv;
   }
-  float* S = P.S + P.path_off[k];
+  float* S = P.S + rq.path_off;
   float score_ss = 0.0f;
 
   int step = 0, i = i2, j = j2, mc = 0, li = i2, lj = j2;
@@ -640,7 +657,7 @@ __global__ void k_backtrace(const BtParams P) {
   }
   HitRec h;
   h.score = best; h.i2 = i2; h.j2 = j2; h.i1 = li; h.j1 = lj; h.nsteps = step;
-  h.matched_cols = mc; h.path_off = (int)P.path_off[k];
+  h.matched_cols = mc; h.path_off = (int)rq.path_off;
   h.hit_score = hs; h.score_ss = score_ss;
   P.hits[k] = h;
 }
@@ -670,12 +687,12 @@ __global__ void k_null_model(long long total_cols, int n, const long long* col_o
 
 // Compact the per-request path strings (capacity Lq+Lt+2 each) to their real lengths before the D2H copy:
 // one thread per request copies nsteps bytes to its compact offset.
-__global__ void k_gather_paths(int n, const HitRec* hits, const long long* src_off, const long long* dst_off,
+__global__ void k_gather_paths(int n, const HitRec* hits, const ReqDesc* reqs, const long long* dst_off,
                                const uint8_t* src, uint8_t* dst) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const int len = hits[k].nsteps;
-  const uint8_t* s = src + src_off[k];
+  const uint8_t* s = src + reqs[k].path_off;
   uint8_t* d = dst + dst_off[k];
   for (int b = 0; b < len; ++b) d[b] = s[b];
 }
@@ -720,25 +737,24 @@ __global__ void k_pack_cols(int n, const int* L, const long long* col_off, const
 
 // Build the job-interleaved operand stream of a plan from the shard's column records: warp per (job, column),
 // lane = the job's lane.  Each lane copies its own 112-byte record (7 x 16 B) of column min(j, Lt) into
-// out[job_jc_off[job] + ((j-1)*7 + k)*32 + lane]: the seven stores of a warp are full 512-byte lines.
+// out[jobs[job].jc_off + ((j-1)*7 + k)*32 + lane]: the seven stores of a warp are full 512-byte lines.
 __global__ void __launch_bounds__(256)
-k_interleave_cols(int njobs, const int* __restrict__ job_target, const int* __restrict__ job_Lmax,
-                  const long long* __restrict__ job_jc_off, const float4* __restrict__ cols,
+k_interleave_cols(const JobDesc* __restrict__ jobs, const int* __restrict__ job_target, const float4* __restrict__ cols,
                   const long long* __restrict__ col_off, const int* __restrict__ Lt, float4* __restrict__ out,
-                  int nm_mode, const int* __restrict__ job_query, const float* __restrict__ q_pav,
-                  const float* __restrict__ t_pav, const float* __restrict__ pb) {
+                  int nm_mode, const float* __restrict__ q_pav, const float* __restrict__ t_pav,
+                  const float* __restrict__ pb) {
   const int job = blockIdx.x;
   const int lane = threadIdx.x & 31;
-  const int Lmax = job_Lmax[job];
+  const int Lmax = jobs[job].Lmax;
   const int t = job_target[job * 32 + lane];
   const int L = Lt[t];
   const float4* src0 = cols + (size_t)col_off[t] * 7;
-  float4* dst0 = out + job_jc_off[job] + lane;
+  float4* dst0 = out + jobs[job].jc_off + lane;
   // nm_mode >= 0: `cols` holds the emissions before the null model; factor it in for this job's query on the way
   // (HMM::IncludeNullModelInHMM, the query-dependent step of PrepareTemplateHMM), so a batch of queries can share one
   // resident raw shard
   float pn[20];
-  if (nm_mode >= 0) null_model_vec(nm_mode, q_pav + (size_t)job_query[job] * 20, t_pav + (size_t)t * 20, pb, pn);
+  if (nm_mode >= 0) null_model_vec(nm_mode, q_pav + (size_t)jobs[job].query * 20, t_pav + (size_t)t * 20, pb, pn);
   for (int j = blockIdx.y * 8 + (threadIdx.x >> 5) + 1; j <= Lmax; j += gridDim.y * 8) {
     const float4* src = src0 + (size_t)(min(j, L) - 1) * 7;
     float4* dst = dst0 + (size_t)(j - 1) * 224;
@@ -752,15 +768,13 @@ k_interleave_cols(int njobs, const int* __restrict__ job_target, const int* __re
 // Rasterise excluded alignments into the cell-off bit words (Viterbi::ExcludeAlignment,
 // src/hhviterbi.cpp:61-77): one thread per excluded path step.
 __global__ void k_celloff_raster(int n_steps, const int* step_req, const int* step_i, const int* step_j,
-                                 const int* req_job, const int* req_lane, const int* req_Lt, const int* req_Lq,
-                                 const int* job_Lmax, const long long* job_co_off, int R,
-                                 uint32_t* co) {
+                                 const ReqDesc* reqs, const JobDesc* jobs, int R, uint32_t* co) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n_steps) return;
-  const int rq = step_req[k];
-  const int job = req_job[rq], lane = req_lane[rq], Lt = req_Lt[rq], Lq = req_Lq[rq];
-  const int Lmax = job_Lmax[job];
-  uint32_t* base = co + job_co_off[job] + lane;
+  const ReqDesc& rq = reqs[step_req[k]];
+  const int Lt = rq.Lt, Lq = rq.Lq;
+  const int Lmax = jobs[rq.job].Lmax;
+  uint32_t* base = co + jobs[rq.job].co_off + rq.lane;
   const int i = step_i[k], j = step_j[k];
   const int W = 40;   // VITERBI_PATH_WIDTH, src/hhdecl.h:50
   for (int ii = max(i - W, 1); ii <= min(i + W, Lq); ++ii) {
@@ -777,22 +791,21 @@ __global__ void k_celloff_raster(int n_steps, const int* step_req, const int* st
 // -excl / -template_excl options): query rows i0..i1 are switched off for every template column, template columns
 // j0..j1 for every query row.  One thread per cell-off word (job, strip, column, lane).
 __global__ void __launch_bounds__(256)
-k_celloff_regions(long long n_words, int njobs, const long long* __restrict__ job_co_off, const int* __restrict__ job_Lmax,
-                  const int* __restrict__ job_nstrips, int R, int nqr, const int* __restrict__ q_lo,
-                  const int* __restrict__ q_hi, int ntr, const int* __restrict__ t_lo, const int* __restrict__ t_hi,
-                  uint32_t* __restrict__ co) {
+k_celloff_regions(long long n_words, int njobs, const JobDesc* __restrict__ jobs, int R, int nqr,
+                  const int* __restrict__ q_lo, const int* __restrict__ q_hi, int ntr, const int* __restrict__ t_lo,
+                  const int* __restrict__ t_hi, uint32_t* __restrict__ co) {
   const long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (w >= n_words) return;
   int lo = 0, hi = njobs - 1;                       // job owning word w
   while (lo < hi) {
     const int mid = (lo + hi + 1) >> 1;
-    if (job_co_off[mid] <= w) lo = mid; else hi = mid - 1;
+    if (jobs[mid].co_off <= w) lo = mid; else hi = mid - 1;
   }
-  const long long rel = w - job_co_off[lo];
-  const int cols1 = job_Lmax[lo] + 1;
+  const long long rel = w - jobs[lo].co_off;
+  const int cols1 = jobs[lo].Lmax + 1;
   const int s = (int)(rel / ((long long)cols1 * 32));
   const int j = (int)((rel / 32) % cols1);
-  if (s >= job_nstrips[lo] || j < 1) return;
+  if (s >= jobs[lo].nstrips || j < 1) return;
   uint32_t m = 0;
   for (int k = 0; k < ntr; ++k) if (j >= t_lo[k] && j <= t_hi[k]) m = 0xFFFFFFFFu;
   for (int k = 0; k < nqr && m != 0xFFFFFFFFu; ++k) {
