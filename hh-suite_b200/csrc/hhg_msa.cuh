@@ -18,6 +18,7 @@
 // host's own RCPPS for every possible argument (n*naa <= 65535*20, integers) at first use and the kernel looks the
 // value up, so the result is bit-identical to the reference running on the same host.
 #pragma once
+#include <algorithm>
 #include <cctype>
 #include <cfloat>
 #include <cstdint>
@@ -36,13 +37,15 @@ namespace hhg {
 constexpr int MSA_ANY = 20, MSA_GAP = 21, MSA_ENDGAP = 22;   // src/hhdecl.h:52-56
 constexpr int MSA_RCP_N = 1 << 21;                            // > 65535 * 20
 constexpr int MSA_MSTATE_THREADS = 128;                       // block size of k_msa_mstate (see the kernel)
+constexpr int MSA_TAIL = 32;                                  // bytes after column L+1 of a row: what Filter2 reads there
 
 // ------------------------------------------------------------------------------------------ host: scanner
 struct MsaHost {
   int N_in = 0, L = 0, stride = 0;
   int kfirst = -1, kss_dssp = -1, ksa_dssp = -1, kss_pred = -1, kss_conf = -1, N_ss = 0;
   std::vector<int8_t> keep, display;     // [N_in] as Alignment::Read leaves them (0 / 1 / 2); nres == 0 -> keep 0
-  std::vector<uint8_t> X;                // [N_in][stride]: code 0..22 of columns 0..L+1, bit 7 = insert after the column
+  std::vector<uint8_t> X;                // [N_in][stride]: code 0..22 of columns 0..L+1, bit 7 = insert after the column,
+                                         // then MSA_TAIL codes of columns L+1.. as Filter2 sees them (see compress)
   std::vector<int32_t> first, last, nres, ksort;   // [N_in]
   std::vector<uint32_t> ins_off;         // [L+2] CSR over columns 0..L of the inserts, ascending sequence index
   std::vector<int32_t> ins_k;
@@ -286,6 +289,7 @@ class MsaScanner {
     std::vector<std::vector<uint16_t>> I(N);
     int L = maxres - 2, unequal = 0;
     std::vector<int> raw_nres;                              // see the M == 2 branch
+    std::vector<std::vector<uint8_t>> tail(N);              // see the M == 2 branch
     // "Too few match states" (:861-880): a file with ONE sequence whose upper-case letters + '-' number fewer than 6
     // is read as if -M first had been given: every letter of that sequence is a match state, '-' columns are not
     bool by_first = M == 3;
@@ -350,6 +354,11 @@ class MsaScanner {
       if (kfirst < 0) return "the alignment contains no master sequence";
       A.kfirst = kfirst;
       L = i;
+      // Compress moves the match columns to the front of each row in place, so beyond column L the rows still hold the
+      // codes of input columns L+1, L+2, ... while Filter2 runs (FrequenciesAndTransitions sets X[k][L+1] = ENDGAP only
+      // afterwards).  Filter2's 32-byte windows reach up to 31 columns past L and count residues found there.
+      for (int q = 0; q < N; ++q)
+        if (A.keep[q] && raw > (size_t)L) tail[q].assign(C[q].begin() + L, C[q].begin() + std::min(raw, (size_t)L + MSA_TAIL));
       // Compress fills nres[] with the residues over ALL input columns here, and Filter2 recomputes it over the match
       // columns only `if (nres == NULL || sizeof(nres) < N_in * sizeof(int))` (:1660), i.e. only when N_in > 2
       if (N <= 2) raw_nres = nr;
@@ -407,7 +416,7 @@ class MsaScanner {
     if (L <= 0) return "the alignment contains no match states";
     if (L == maxres - 2) return "more than maxres-2 match columns";
     A.L = L;
-    A.stride = (L + 2 + 3) & ~3;
+    A.stride = (L + 2 + MSA_TAIL + 3) & ~3;
     A.X.assign((size_t)N * A.stride, (uint8_t)MSA_GAP);      // initX: rows are GAP beyond what was written
     A.ins_off.assign((size_t)L + 2, 0);
     for (int q = 0; q < N; ++q) {
@@ -423,6 +432,7 @@ class MsaScanner {
       // takes part in Filter2 (both codes are "no residue"), so column L+1 carries ENDGAP from the start and column 0
       // is never read as a predecessor (k_msa_mstate treats it as "not in the sub-alignment")
       row[L + 1] = MSA_ENDGAP;
+      std::copy(tail[q].begin(), tail[q].end(), row + L + 2);  // GAP where the reference's row holds no residue there
     }
     // first / last / nres over ALL rows, nres == 0 -> keep 0 (Filter2 :1647-1676)
     A.first.resize(N); A.last.resize(N); A.nres.resize(N); A.ksort.resize(N);
@@ -697,10 +707,17 @@ k_msa_filter(MsaArrays A, const __grid_constant__ MsaFilterParams P) {
         for (int w = (f_kj & ~3) + 4 * lane; w <= l_kj; w += 128) {
           const uint32_t a4 = *reinterpret_cast<const uint32_t*>(XK + w) & 0x7f7f7f7fu;
           const uint32_t b4 = *reinterpret_cast<const uint32_t*>(XJ + w) & 0x7f7f7f7fu;
-          const uint32_t both = __vcmpltu4(a4, 0x14141414u) & __vcmpltu4(b4, 0x14141414u);
+          uint32_t both = __vcmpltu4(a4, 0x14141414u) & __vcmpltu4(b4, 0x14141414u);
+          if (w + 3 > L) both &= (1u << 8 * (L + 1 - w)) - 1u;   // bytes past column L: the tail below
           const uint32_t ne = ~__vcmpeq4(a4, b4);
           cov += __popc(both) >> 3;
           diff += __popc(both & ne) >> 3;
+        }
+        // the reference's last window ends at the next multiple of 32 after l_kj; past column L it reads what Compress
+        // left in the rows (input columns with -M <percent>, GAP otherwise), stored after column L+1 of each row
+        if (lane < (l_kj / 32 + 1) * 32 - 1 - L) {
+          const int a = XK[L + 2 + lane] & 0x7f, b = XJ[L + 2 + lane] & 0x7f;
+          if (a < 20 && b < 20) { ++cov; diff += a != b; }
         }
 #pragma unroll
         for (int o = 16; o; o >>= 1) { diff += __shfl_xor_sync(0xffffffffu, diff, o); cov += __shfl_xor_sync(0xffffffffu, cov, o); }

@@ -135,3 +135,34 @@ def test_emulated_kernels_with_other_match_state_rules(emul, refshim, tmp_path, 
             _cmp(_run(emul, refshim, t, M=M, Mgaps=Mgaps), refshim.msa_to_hmm(str(path)), f"fasta {k} M={M}/{Mgaps}")
     finally:
         refshim.set_M(1, 50)
+
+
+def test_emulated_kernels_on_random_alignments(emul, refshim, tmp_path):
+    """15 seeded alignments of tests/msa_cases.py's generator: tiny and typical A3M records under M = 1 and aligned
+    FASTA under -M 50, -M 25 and -M first, each with random filter options and weighting mode."""
+    rng = np.random.default_rng(15)
+    specs = [("tiny", 1, 50)] * 6 + [("typical", 1, 50)] * 3 + [("fasta", 2, 50), ("fasta", 2, 25), ("fasta", 3, 50)] * 2
+    try:
+        for k, (kind, M, Mg) in enumerate(specs):
+            t = msa_cases.random_fasta(rng, M, Mg) if kind == "fasta" else msa_cases.random_alignment(rng, kind)
+            filt, wg = msa_cases.random_filter(rng)
+            path = tmp_path / f"r{k}.a3m"
+            path.write_bytes(t)
+            refshim.set_M(M, Mg)
+            got = _run(emul, refshim, t, filt=filt, wg=wg, M=M, Mgaps=Mg)     # before the reference: it exits on refusals
+            _cmp(got, refshim.msa_to_hmm(str(path), filt=filt, wg=wg), f"{kind} {k} M={M}/{Mg} {filt} wg={wg}")
+    finally:
+        refshim.set_M(1, 50)
+
+
+def test_emulated_kernels_on_fixed_match_state_rule_cases(emul, refshim, tmp_path):
+    try:
+        for k, (t, M, Mg, filt) in enumerate(msa_cases.MRULE_CASES):
+            path = tmp_path / f"c{k}.fas"
+            path.write_bytes(t)
+            refshim.set_M(M, Mg)
+            for wg in (0, 1):
+                got = _run(emul, refshim, t, filt=filt, wg=wg, M=M, Mgaps=Mg)
+                _cmp(got, refshim.msa_to_hmm(str(path), filt=filt, wg=wg), f"case {k} wg={wg}")
+    finally:
+        refshim.set_M(1, 50)

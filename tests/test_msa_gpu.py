@@ -63,6 +63,23 @@ def test_global_weights(hhg, gpu_ctx, refshim, tmp_path):
         _cmp(got, ref, f"case {k} wg=1")
 
 
+def test_fixed_match_state_rule_cases(hhg, gpu_ctx, refshim, tmp_path):
+    """msa_cases.MRULE_CASES: alignments read with -M <percent> / -M first that once differed from the reference."""
+    pb, S = refshim.pb(), refshim.S()
+    try:
+        for k, (t, M, Mg, filt) in enumerate(msa_cases.MRULE_CASES):
+            path = tmp_path / f"c{k}.fas"
+            path.write_bytes(t)
+            refshim.set_M(M, Mg)
+            for wg in (0, 1):
+                mp = hhg.capi.MsaParams.defaults(M=M, Mgaps=Mg, max_seqid=filt[0], coverage=filt[1], qid=filt[2], qsc=filt[3],
+                                                 Ndiff=filt[4], wg=wg)
+                _cmp(hhg.capi.msa_to_hmm(gpu_ctx, t, pb, S=S, mp=mp), refshim.msa_to_hmm(str(path), filt=filt, wg=wg),
+                     f"case {k} wg={wg}")
+    finally:
+        refshim.set_M(1, 50)
+
+
 def test_reciprocal_table_is_the_hosts(hhg, gpu_ctx, refshim):
     """1-sequence sub-alignments put 1/(1*1) = RCPPS(1) into every weight: check the library saw the same value the
     reference build gets from simdf32_rcp on this host."""

@@ -16,63 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from hhsuite_b200 import capi, synth  # noqa: E402
 from oracle.binding import RefShim  # noqa: E402
-
-AA = "ARNDCQEGHILKMFPSTWYV"
-
-
-def rand_a3m(rng):
-    L = int(rng.integers(1, 40)); n = int(rng.integers(0, 12))
-    alpha = AA + "XBZUJO"
-    lines = []
-    if rng.random() < 0.3:
-        lines.append("#NAME some description")
-    if rng.random() < 0.3:
-        lines += [">ss_pred", "".join(rng.choice(list("HEC-"), L))]
-        if rng.random() < 0.6:
-            lines += [">ss_conf", "".join(rng.choice(list("0123456789"), L))]
-
-    def row(first=False):
-        out = []
-        if rng.random() < 0.2:
-            out.append("".join(rng.choice(list(AA.lower()), int(rng.integers(1, 4)))))
-        for _ in range(L):
-            out.append(rng.choice(list(alpha)) if rng.random() < 0.85 or first else "-")
-            if rng.random() < 0.1:
-                out.append("".join(rng.choice(list(AA.lower()), int(rng.integers(1, 4)))))
-            if rng.random() < 0.03:
-                out.append(".")
-        s = "".join(out)
-        return s if any(ch.isalpha() for ch in s) else "A" + s[1:]
-    lines += [">master" if rng.random() < 0.9 else ">cons_consensus", row(True)]
-    for k in range(n):
-        lines.append(f">s{k}")
-        s = row()
-        if rng.random() < 0.3 and len(s) > 4:
-            c = int(rng.integers(1, len(s) - 1)); lines += [s[:c], s[c:]]
-        else:
-            lines.append(s)
-    eol = "\r\n" if rng.random() < 0.2 else "\n"
-    return (eol.join(lines) + eol).encode()
-
-
-def rand_fasta(rng):
-    L = int(rng.integers(3, 60)); n = int(rng.integers(1, 15))
-    gapcol = rng.random(L) < 0.25
-
-    def row(first=False):
-        out = []
-        for i in range(L):
-            pg = 0.7 if gapcol[i] else 0.08
-            if rng.random() < pg and not (first and rng.random() < 0.5):
-                out.append("-")
-            else:
-                c = rng.choice(list(AA + "X")); out.append(c.lower() if rng.random() < 0.05 else c)
-        s = "".join(out)
-        return s if any(ch.isalpha() for ch in s) else "A" + s[1:]
-    lines = [">master", row(True)]
-    for k in range(n):
-        lines += [f">s{k}", row()]
-    return ("\n".join(lines) + "\n").encode()
+from tests.msa_cases import rand_a3m, rand_fasta  # noqa: E402
 
 
 def same_scan(a, o):
