@@ -127,12 +127,13 @@ class Crf:
         _ck(load().hhg_crf_tail_host(self.h, L, score.ctypes.data, _p(f, c_f32p), _p(neff_m, c_f32p), C.byref(admix), _p(p, c_f32p)))
         return p
 
-    def pseudocounts(self, f, neff_m, neff_hmm, pb, admix):
-        """hhg_query_context_pseudocounts -> (p[(L+2),20] incl. rows 0 / L+1 = pav, pav[20])."""
+    def pseudocounts(self, f, neff_m, neff_hmm, pb, admix, want_pav=True):
+        """hhg_query_context_pseudocounts -> (p[(L+2),20] incl. rows 0 / L+1 = pav, pav[20]); without want_pav the
+        background step is skipped: rows 0 and L+1 stay zero and pav is None."""
         f = np.ascontiguousarray(f, np.float32); neff_m = np.ascontiguousarray(neff_m, np.float32)
         pb = np.ascontiguousarray(pb, np.float32)
         L = f.shape[0] - 2
-        p = np.zeros((L + 2, 20), np.float32); pav = np.zeros(20, np.float32)
+        p = np.zeros((L + 2, 20), np.float32); pav = np.zeros(20, np.float32) if want_pav else None
         _ck(self.ctx.L.hhg_query_context_pseudocounts(self.ctx.h, self.h, L, _p(f, c_f32p), _p(neff_m, c_f32p), float(neff_hmm),
                                                       _p(pb, c_f32p), C.byref(admix), _p(p, c_f32p), _p(pav, c_f32p)))
         return p, pav

@@ -1247,6 +1247,11 @@ int hhg_query_context_pseudocounts(hhg_ctx* ctx, const hhg_crf* crf, int32_t L, 
   if (!ctx || !crf || L < 1 || !f || !neff_m || !admix || !p) return fail(HHG_EINVAL, "hhg_query_context_pseudocounts: bad argument");
   if (admix->kind < 0 || admix->kind > 2) return fail(HHG_EINVAL, "hhg_query_context_pseudocounts: admixture kind %d (0 constant, 1 CS-BLAST, 2 HHsearch)", admix->kind);
   if (pav && !pb) return fail(HHG_EINVAL, "hhg_query_context_pseudocounts: pav needs the background pb");
+  // the result only feeds hhg_query_set, which takes Lq <= 32767; k_crf_scores runs one block row per column
+  if (L > 32767) return fail(HHG_EINVAL, "hhg_query_context_pseudocounts: L = %d exceeds the query limit of 32767 columns", L);
+  if (crf->device != ctx->device)
+    return fail(HHG_EINVAL, "hhg_query_context_pseudocounts: the CRF was created on device %d, the context is on device %d",
+                crf->device, ctx->device);
   CK(cudaSetDevice(ctx->device));
   const int K = crf->host.K, W = crf->host.W;
   // HMM::fillCountProfile (src/hhhmm.cpp:1843-1849): counts = f * Neff_M (float product), neff = Neff_M

@@ -65,7 +65,10 @@ inline std::string crf_parse(const char* text, int64_t len, CrfHost* out) {
   int size = 0, wlen = 0;
   if (!next_line(ln) || !read_int(ln, "SIZE", &size)) return "unable to parse CRF 'SIZE'";
   if (!next_line(ln) || !read_int(ln, "LENG", &wlen)) return "unable to parse CRF 'LENG'";
-  if (size < 1 || wlen < 1 || !(wlen & 1) || wlen > 63) return "bad CRF size / window length";
+  if (size < 1) return "CRF SIZE " + std::to_string(size) + " is not a positive number of states";
+  // k_crf_scores stages the window in a 64-column shared-memory tile; the reference's reader asserts on even windows
+  if (wlen < 1 || !(wlen & 1) || wlen > 63)
+    return "CRF window length " + std::to_string(wlen) + " is not supported: the window must be odd and 1..63 columns";
   C.K = size; C.W = wlen;
   C.bias.assign(size, 0.0);
   C.w.assign((size_t)wlen * 20 * size, 0.0);

@@ -224,6 +224,8 @@ int hhg_db_create_a3m(hhg_ctx* ctx, int n, const char* data, const int64_t* off,
  * does, so it runs on the library's host threads: every output equals the reference's, bit for bit.
  *   f[(L+2)*20] frequencies without pseudocounts (HMM::f, e.g. from hhg_msa_to_hmm), neff_m[L+1] (Neff_M),
  *   p[(L+2)*20] out: rows 1..L; with pav != NULL also CalculateAminoAcidBackground (pb, neff_hmm): pav and rows 0, L+1.
+ * Limits: windows are odd and at most 63 columns (hhg_crf_create refuses others); 1 <= L <= 32767, the query limit of
+ * hhg_query_set; crf must have been created on ctx's device.  Each is HHG_EINVAL before anything is allocated or launched.
  * Target-Neff admixture (par...target_neff >= 1) is not built (default 0). */
 typedef struct hhg_crf hhg_crf;
 typedef struct hhg_admix { int32_t kind; double pca, pcb, pcc; } hhg_admix;   /* kind 0 constant, 1 CS-BLAST, 2 HHsearch */

@@ -404,6 +404,49 @@ class RefShim:
         self.lib.hhref_context_pc(L, _p(f, c_f32p), _p(neff_m, c_f32p), float(neff_hmm), engine, _p(p, c_f32p), _p(pav, c_f32p))
         return p, pav
 
+    # cs::Admix classes by name; the library's hhg_admix.kind numbers them 0 constant, 1 CS-BLAST, 2 HHsearch, the
+    # reference's Pseudocounts::Admix enum 1 Constant, 2 HHsearch, 3 CSBlast -- neither number crosses this binding.
+    ADMIX_CLASSES = ("constant", "csblast", "hhsearch")
+
+    def _crf_error(self):
+        self.lib.hhref_crf_error.restype = C.c_char_p
+        return self.lib.hhref_crf_error().decode(errors="replace")
+
+    def crf_text_state(self, text, k):
+        """State k of the context library `text` as the reference's cs::Crf reader reads it -> (n_states, pc[20], bias,
+        w[wlen, 20]).  Raises ValueError with the reader's message when it refuses the text."""
+        wlen = C.c_int(); pc = np.zeros(20, np.float64); b = C.c_double()
+        fn = self.lib.hhref_crf_text_state
+        fn.argtypes = [C.c_char_p, C.c_longlong, C.c_int, C.POINTER(C.c_int), C.c_void_p, C.POINTER(C.c_double), C.c_void_p]
+        n = fn(text, len(text), k, C.byref(wlen), pc.ctypes.data, C.byref(b), None)
+        if n == -1:
+            raise ValueError(f"the reference's CRF reader refused the text: {self._crf_error()}")
+        if n < 0:
+            raise IndexError(k)
+        w = np.zeros((wlen.value, 20), np.float64)
+        fn(text, len(text), k, C.byref(wlen), pc.ctypes.data, C.byref(b), w.ctypes.data)
+        return n, pc, b.value, w
+
+    def context_pc_crf(self, text, f, neff_m, neff_hmm, admix, pca, pcb=0.0, pcc=1.0):
+        """context_pc with the library (`.crf` text) and the admixture given explicitly: admix names the cs::Admix class,
+        one of ADMIX_CLASSES ("constant": pca; "csblast": pca, pcb; "hhsearch": pca, pcb, pcc)."""
+        if admix not in self.ADMIX_CLASSES:
+            raise ValueError(f"admixture class {admix!r} is not one of {self.ADMIX_CLASSES}")
+        f = np.ascontiguousarray(f, np.float32); neff_m = np.ascontiguousarray(neff_m, np.float32)
+        L = f.shape[0] - 2
+        p = np.zeros((L + 2, 20), np.float32); pav = np.zeros(20, np.float32)
+        fn = self.lib.hhref_context_pc_crf
+        fn.argtypes = [C.c_char_p, C.c_longlong, C.c_char_p, C.c_double, C.c_double, C.c_double, C.c_int, c_f32p, c_f32p,
+                       C.c_float, c_f32p, c_f32p]
+        r = fn(text, len(text), admix.encode(), float(pca), float(pcb), float(pcc), L, _p(f, c_f32p), _p(neff_m, c_f32p),
+               float(neff_hmm), _p(p, c_f32p), _p(pav, c_f32p))
+        if r == -1:
+            raise ValueError(f"the reference's CRF reader refused the text: {self._crf_error()}")
+        if r == -3:
+            raise ValueError(f"L = {L} does not fit maxres {self.maxres}")
+        assert r == L, r
+        return p, pav
+
     def set_mac_exclstr(self, q="", t=""):
         """par.exclstr / par.template_exclstr (-excl / -template_excl) for the following mac_realign calls."""
         self.lib.hhref_set_mac_exclstr.argtypes = [C.c_char_p, C.c_char_p]

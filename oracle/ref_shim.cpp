@@ -831,3 +831,85 @@ extern "C" const unsigned char* hhref_crf_text(long long* len) {
   *len = (long long)context_data_crf_len;
   return context_data_crf;
 }
+
+// A context library given as text (what `-contxt file.crf` reads), parsed by cs::Crf's own reader through fmemopen as
+// InitializePseudocountsEngine does (src/hhfunc.cpp:221-228).  Parsed libraries are cached by content, so a 4000-state
+// text is read once per process; a text the reader refuses is cached with the reader's message.
+namespace {
+struct CrfByText {
+  std::string text, err;
+  std::unique_ptr<cs::Crf<cs::AA>> crf;
+};
+std::vector<std::unique_ptr<CrfByText>> g_crf_texts;
+std::string g_crf_err;
+
+const cs::Crf<cs::AA>* crf_from_text(const char* text, long long len) {
+  for (auto& e : g_crf_texts)
+    if ((long long)e->text.size() == len && memcmp(e->text.data(), text, (size_t)len) == 0) {
+      g_crf_err = e->err;
+      return e->crf.get();
+    }
+  std::unique_ptr<CrfByText> e(new CrfByText());
+  e->text.assign(text, (size_t)len);
+  FILE* fin = fmemopen((void*)e->text.data(), e->text.size(), "r");
+  try {
+    e->crf.reset(new cs::Crf<cs::AA>(fin));
+  } catch (const std::exception& ex) {        // cs::Exception, what the reader throws
+    e->err = ex.what();
+    if (e->err.empty()) e->err = "refused";
+  }
+  fclose(fin);
+  if (g_crf_texts.size() >= 16) g_crf_texts.erase(g_crf_texts.begin());
+  g_crf_texts.push_back(std::move(e));
+  g_crf_err = g_crf_texts.back()->err;
+  return g_crf_texts.back()->crf.get();
+}
+}  // namespace
+
+// the message of the last refused text (empty when it was accepted)
+extern "C" const char* hhref_crf_error() { return g_crf_err.c_str(); }
+
+// state k of the library in `text`: *wlen, pc[20], bias, w[wlen*20] (w may be NULL).  Returns the number of states,
+// -1 when the reader refused the text (hhref_crf_error), -2 when k is out of range.
+extern "C" int hhref_crf_text_state(const char* text, long long len, int k, int* wlen, double* pc, double* bias, double* w) {
+  const cs::Crf<cs::AA>* crf = crf_from_text(text, len);
+  if (!crf) return -1;
+  if (k < 0 || k >= (int)crf->size()) return -2;
+  const cs::CrfState<cs::AA>& s = (*crf)[k];
+  *wlen = (int)s.context_weights.length();
+  for (int a = 0; a < 20; ++a) pc[a] = s.pc[a];
+  *bias = s.bias_weight;
+  if (w)
+    for (size_t j = 0; j < s.context_weights.length(); ++j)
+      for (int a = 0; a < 20; ++a) w[j * 20 + a] = s.context_weights[j][a];
+  return (int)crf->size();
+}
+
+// hhref_context_pc with the library and the admixture given explicitly: cs::CrfPseudocounts on the library in `text`
+// and one of cs::ConstantAdmix(pca) ("constant"), cs::CSBlastAdmix(pca, pcb) ("csblast") or
+// cs::HHsearchAdmix(pca, pcb, pcc) ("hhsearch"), then HMM::AddContextSpecificPseudocounts + CalculateAminoAcidBackground.
+// Returns L, -1 when the reader refused the text, -2 for an unknown admixture class, -3 when L + 2 > maxres.
+extern "C" int hhref_context_pc_crf(const char* text, long long len, const char* admix, double pca, double pcb, double pcc,
+                                    int L, const float* f, const float* neff_m, float neff_hmm, float* p, float* pav) {
+  const cs::Crf<cs::AA>* crf = crf_from_text(text, len);
+  if (!crf) return -1;
+  std::unique_ptr<cs::Admix> mode;
+  if (!strcmp(admix, "constant")) mode.reset(new cs::ConstantAdmix(pca));
+  else if (!strcmp(admix, "csblast")) mode.reset(new cs::CSBlastAdmix(pca, pcb));
+  else if (!strcmp(admix, "hhsearch")) mode.reset(new cs::HHsearchAdmix(pca, pcb, pcc));
+  else return -2;
+  if (L + 2 > g->maxres) return -3;
+  cs::CrfPseudocounts<cs::AA> engine(*crf);
+  HMM* h = new HMM(MAXSEQDIS, g->maxres);
+  h->L = L;
+  h->has_pseudocounts = false;
+  h->Neff_HMM = neff_hmm;
+  for (int i = 0; i <= L + 1; ++i) for (int a = 0; a < 20; ++a) h->f[i][a] = f[(size_t)i * 20 + a];
+  for (int i = 0; i <= L; ++i) h->Neff_M[i] = neff_m[i];
+  h->AddContextSpecificPseudocounts(&engine, mode.get());
+  h->CalculateAminoAcidBackground(g->pb);
+  for (int i = 0; i <= L + 1; ++i) for (int a = 0; a < 20; ++a) p[(size_t)i * 20 + a] = h->p[i][a];
+  for (int a = 0; a < 20; ++a) pav[a] = h->pav[a];
+  delete h;
+  return L;
+}
