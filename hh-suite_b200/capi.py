@@ -47,7 +47,7 @@ SYMBOLS = ["hhg_last_error", "hhg_ctx_create", "hhg_ctx_destroy", "hhg_ctx_sync"
            "hhg_msa_params_default", "hhg_a3m_scan", "hhg_a3m_parse", "hhg_msa_to_hmm", "hhg_db_create_a3m", "hhg_query_from_a3m",
            "hhg_ca3m_scan", "hhg_ca3m_parse", "hhg_ca3m_to_hmm", "hhg_db_create_ca3m",
            "hhg_crf_create", "hhg_crf_destroy", "hhg_crf_info", "hhg_query_context_pseudocounts", "hhg_crf_parse_host",
-           "hhg_crf_state", "hhg_crf_tail_host"]
+           "hhg_crf_state", "hhg_crf_tail_host", "hhg_context_library_create", "hhg_context_library_parse_host"]
 
 
 class PrepParams(C.Structure):
@@ -97,12 +97,16 @@ class Crf:
     """hhg_crf: the context library of the CRF pseudocounts (text of a `.crf` file, e.g. HH-suite's context_data.crf)."""
 
     def __init__(self, ctx, text: bytes):
+        self._open(ctx, "hhg_crf_parse_host", "hhg_crf_create", text)
+
+    def _open(self, ctx, parse_host, create, text, *args):
+        """Host-only handle (ctx None) or one uploaded to ctx's device, then its size."""
         self.h = C.c_void_p()
         self.ctx = ctx
         if ctx is None:
-            _ck(load().hhg_crf_parse_host(text, len(text), C.byref(self.h)))
+            _ck(getattr(load(), parse_host)(text, len(text), *args, C.byref(self.h)))
         else:
-            _ck(ctx.L.hhg_crf_create(ctx.h, text, len(text), C.byref(self.h)))
+            _ck(getattr(ctx.L, create)(ctx.h, text, len(text), *args, C.byref(self.h)))
         n = np.zeros(1, np.int32); w = np.zeros(1, np.int32)
         _ck(load().hhg_crf_info(self.h, _p(n, c_i32p), _p(w, c_i32p), None))
         self.n_states, self.window = int(n[0]), int(w[0])
@@ -142,6 +146,17 @@ class Crf:
         if self.h:
             load().hhg_crf_destroy(self.h)
             self.h = None
+
+
+class ContextLibrary(Crf):
+    """hhg_crf of the generative engine: a context library (text of a `.lib` file, e.g. HH-suite's context_data.lib)
+    with the window weights of -csw / -csb.  hhblits keeps those as floats, so the defaults are float32(1.6) and
+    float32(0.85).  state(k) gives a profile's log-probabilities and log prior; pc() the central columns."""
+
+    def __init__(self, ctx, text: bytes, weight_center=float(np.float32(1.6)), weight_decay=float(np.float32(0.85))):
+        self.weight_center, self.weight_decay = float(weight_center), float(weight_decay)
+        self._open(ctx, "hhg_context_library_parse_host", "hhg_context_library_create", text, self.weight_center,
+                   self.weight_decay)
 
 
 class SeqDb(C.Structure):
@@ -296,6 +311,8 @@ def load():
     L.hhg_crf_info.argtypes = [C.c_void_p, c_i32p, c_i32p, C.c_void_p]
     L.hhg_crf_state.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_double)]
     L.hhg_crf_tail_host.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, c_f32p, c_f32p, C.c_void_p, c_f32p]
+    L.hhg_context_library_create.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_double, C.c_double, C.POINTER(C.c_void_p)]
+    L.hhg_context_library_parse_host.argtypes = [C.c_char_p, C.c_int64, C.c_double, C.c_double, C.POINTER(C.c_void_p)]
     L.hhg_query_context_pseudocounts.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, c_f32p, c_f32p, C.c_float, c_f32p,
                                                  C.c_void_p, c_f32p, c_f32p]
     L.hhg_ca3m_scan.argtypes = [C.c_char_p, C.c_int64, C.c_void_p, C.c_void_p, c_i32p, c_i32p]

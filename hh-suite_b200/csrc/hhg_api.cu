@@ -1178,25 +1178,44 @@ int hhg_query_from_a3m(hhg_ctx* ctx, const char* rec, int64_t len, const hhg_msa
 
 // ---------------------------------------------------------------------------------------------------------------
 // Context-specific pseudocounts of the query (hhg_crf.cuh)
+// One handle for either engine, as the reference holds one Pseudocounts* whatever the file type: host.library tells
+// which score kernel runs (k_crf_scores or k_lib_scores) and where the tail's maximum starts.
 struct hhg_crf {
   int device = 0;
   hhg::CrfHost host;
-  DevBuf<double> d_w, d_bias;
+  DevBuf<double> d_w, d_bias, d_ww;
 };
+
+static int crf_upload(hhg_ctx* ctx, std::unique_ptr<hhg_crf>& c, hhg_crf** out) {
+  CK(cudaSetDevice(ctx->device));
+  c->device = ctx->device;
+  CK(c->d_w.alloc(c->host.w.size())); CK(c->d_bias.alloc(c->host.bias.size()));
+  CK(cudaMemcpyAsync(c->d_w.p, c->host.w.data(), c->host.w.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(c->d_bias.p, c->host.bias.data(), c->host.bias.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+  if (c->host.library) {
+    CK(c->d_ww.alloc(c->host.ww.size()));
+    CK(cudaMemcpyAsync(c->d_ww.p, c->host.ww.data(), c->host.ww.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  CK(cudaStreamSynchronize(ctx->stream));
+  *out = c.release();
+  return HHG_OK;
+}
 
 int hhg_crf_create(hhg_ctx* ctx, const char* text, int64_t len, hhg_crf** out) {
   if (!ctx || !text || len <= 0 || !out) return fail(HHG_EINVAL, "hhg_crf_create: bad argument");
   std::unique_ptr<hhg_crf> c(new hhg_crf());
   const std::string msg = crf_parse(text, len, &c->host);
   if (!msg.empty()) return fail(HHG_EINVAL, "hhg_crf_create: %s", msg.c_str());
-  CK(cudaSetDevice(ctx->device));
-  c->device = ctx->device;
-  CK(c->d_w.alloc(c->host.w.size())); CK(c->d_bias.alloc(c->host.bias.size()));
-  CK(cudaMemcpyAsync(c->d_w.p, c->host.w.data(), c->host.w.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(c->d_bias.p, c->host.bias.data(), c->host.bias.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  *out = c.release();
-  return HHG_OK;
+  return crf_upload(ctx, c, out);
+}
+
+int hhg_context_library_create(hhg_ctx* ctx, const char* text, int64_t len, double weight_center, double weight_decay,
+                               hhg_crf** out) {
+  if (!ctx || !text || len <= 0 || !out) return fail(HHG_EINVAL, "hhg_context_library_create: bad argument");
+  std::unique_ptr<hhg_crf> c(new hhg_crf());
+  const std::string msg = lib_parse(text, len, weight_center, weight_decay, &c->host);
+  if (!msg.empty()) return fail(HHG_EINVAL, "hhg_context_library_create: %s", msg.c_str());
+  return crf_upload(ctx, c, out);
 }
 
 int hhg_crf_destroy(hhg_crf* crf) { delete crf; return HHG_OK; }
@@ -1208,6 +1227,8 @@ int hhg_crf_info(const hhg_crf* crf, int32_t* n_states, int32_t* window, double*
   return HHG_OK;
 }
 
+static double crf_tail_start(const hhg::CrfHost& h) { return h.library ? -FLT_MAX : -DBL_MAX; }
+
 // Host only: the per-column tail of hhg_query_context_pseudocounts on caller-supplied context scores
 // (score[L*K], what k_crf_scores produces), for inspection and CPU-side tests.
 int hhg_crf_tail_host(const hhg_crf* crf, int32_t L, double* score, const float* f, const float* neff_m, const hhg_admix* admix,
@@ -1217,8 +1238,8 @@ int hhg_crf_tail_host(const hhg_crf* crf, int32_t L, double* score, const float*
   for (int i = 0; i < L; ++i) {
     double cnt[20];
     for (int a = 0; a < 20; ++a) cnt[a] = f[(size_t)(i + 1) * 20 + a] * neff_m[i + 1];
-    crf_column_tail(K, score + (size_t)i * K, crf->host.pc.data(), cnt, (double)neff_m[i + 1], admix->kind, admix->pca, admix->pcb,
-                    admix->pcc, p + (size_t)(i + 1) * 20);
+    crf_column_tail(K, crf_tail_start(crf->host), score + (size_t)i * K, crf->host.pc.data(), cnt, (double)neff_m[i + 1],
+                    admix->kind, admix->pca, admix->pcb, admix->pcc, p + (size_t)(i + 1) * 20);
   }
   return HHG_OK;
 }
@@ -1229,6 +1250,15 @@ int hhg_crf_parse_host(const char* text, int64_t len, hhg_crf** out) {
   std::unique_ptr<hhg_crf> c(new hhg_crf());
   const std::string msg = crf_parse(text, len, &c->host);
   if (!msg.empty()) return fail(HHG_EINVAL, "hhg_crf_parse_host: %s", msg.c_str());
+  *out = c.release();
+  return HHG_OK;
+}
+
+int hhg_context_library_parse_host(const char* text, int64_t len, double weight_center, double weight_decay, hhg_crf** out) {
+  if (!text || len <= 0 || !out) return fail(HHG_EINVAL, "hhg_context_library_parse_host: bad argument");
+  std::unique_ptr<hhg_crf> c(new hhg_crf());
+  const std::string msg = lib_parse(text, len, weight_center, weight_decay, &c->host);
+  if (!msg.empty()) return fail(HHG_EINVAL, "hhg_context_library_parse_host: %s", msg.c_str());
   *out = c.release();
   return HHG_OK;
 }
@@ -1250,7 +1280,8 @@ int hhg_query_context_pseudocounts(hhg_ctx* ctx, const hhg_crf* crf, int32_t L, 
   // the result only feeds hhg_query_set, which takes Lq <= 32767; k_crf_scores runs one block row per column
   if (L > 32767) return fail(HHG_EINVAL, "hhg_query_context_pseudocounts: L = %d exceeds the query limit of 32767 columns", L);
   if (crf->device != ctx->device)
-    return fail(HHG_EINVAL, "hhg_query_context_pseudocounts: the CRF was created on device %d, the context is on device %d",
+    return fail(HHG_EINVAL, "hhg_query_context_pseudocounts: the %s was created on device %d, the context is on device %d",
+                crf->host.library ? "context library" : "CRF",
                 crf->device, ctx->device);
   CK(cudaSetDevice(ctx->device));
   const int K = crf->host.K, W = crf->host.W;
@@ -1276,14 +1307,18 @@ int hhg_query_context_pseudocounts(hhg_ctx* ctx, const hhg_crf* crf, int32_t L, 
     st.h_n = ns;
   }
   CK(cudaMemcpyAsync(st.counts.p, counts.data(), counts.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-  k_crf_scores<<<dim3((K + 255) / 256, L), 256, 0, ctx->stream>>>(L, K, W, crf->d_w.p, crf->d_bias.p, st.counts.p, st.score.p);
+  const dim3 grid((K + 255) / 256, L);
+  if (crf->host.library)
+    k_lib_scores<<<grid, 256, 0, ctx->stream>>>(L, K, W, crf->d_w.p, crf->d_bias.p, crf->d_ww.p, st.counts.p, st.score.p);
+  else
+    k_crf_scores<<<grid, 256, 0, ctx->stream>>>(L, K, W, crf->d_w.p, crf->d_bias.p, st.counts.p, st.score.p);
   ctx->launches++;
   CK(cudaGetLastError());
   double* score = st.h_score;
   CK(cudaMemcpyAsync(score, st.score.p, ns * 8, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   host_for(L, [&](int i) {
-    crf_column_tail(K, score + (size_t)i * K, crf->host.pc.data(), counts.data() + (size_t)i * 20, neff[i],
+    crf_column_tail(K, crf_tail_start(crf->host), score + (size_t)i * K, crf->host.pc.data(), counts.data() + (size_t)i * 20, neff[i],
                     admix->kind, admix->pca, admix->pcb, admix->pcc, p + (size_t)(i + 1) * 20);
     return std::string();
   });

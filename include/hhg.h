@@ -214,6 +214,8 @@ int hhg_db_create_a3m(hhg_ctx* ctx, int n, const char* data, const int64_t* off,
                       const hhg_msa_params* mp, const float* S, const float* pb, const hhg_prep_params* pp,
                       const float* R, hhg_db** out);
 /* ---- context-specific pseudocounts of the query (SURVEY 8a row a12, the DEFAULT branch of PrepareQueryHMM) ------------
+ * Two engines, as in the reference: the CRF below (a `.crf` file, the default) and the context library after
+ * hhg_crf_tail_host (any other file given to -contxt); both use the hhg_crf handle.
  * Replaces HMM::AddContextSpecificPseudocounts (src/hhhmm.cpp:1820-1849) = cs::Pseudocounts::AddTo(count profile, admix)
  * with the CRF engine (src/cs/crf_pseudocounts-inl.h:74-110, src/cs/pseudocounts-inl.h:41-73), used twice per query by
  * hhblits: for the query HMM (par.pc_hhm_context_engine: HHsearch admixture 0.9 / 4.0 / 1.0) and for the prefilter
@@ -240,6 +242,24 @@ int hhg_crf_parse_host(const char* text, int64_t len, hhg_crf** out);
 int hhg_crf_state(const hhg_crf* crf, int32_t k, double* w, double* bias);
 int hhg_crf_tail_host(const hhg_crf* crf, int32_t L, double* score, const float* f, const float* neff_m, const hhg_admix* admix,
                       float* p);
+/* The generative engine: a context library (`-contxt` with any file that is not a `.crf`; HH-suite ships
+ * data/context_data.lib: 4000 profiles, window 13).  InitializePseudocountsEngine (src/hhfunc.cpp:229-236) reads it with
+ * cs::ContextLibrary, applies TransformToLog and builds cs::LibraryPseudocounts(lib, par.csw, par.csb) for both
+ * engines; the handle this returns stands for that engine and goes to every hhg_crf_* call above and to
+ * hhg_query_context_pseudocounts, with the same limits and the same bit-for-bit results.  The context scores are the
+ * window-weighted emission scores of cs::Emission (src/cs/emission.h:87-103): window weights weight_center and
+ * weight_center * weight_decay^d at distance d.  par.csw / par.csb are floats (src/hhdecl.h:260-261, defaults 1.6f and
+ * 0.85f), so pass (double)1.6f and (double)0.85f to get what hhblits computes, not 1.6 and 0.85.  hhg_crf_state gives a
+ * profile's log-probabilities in w and its log prior in bias; hhg_crf_info's pc is its central column in linear space.
+ * Texts the reference reads but this library refuses (HHG_EINVAL, naming the profile and, where relevant, the
+ * column): even windows and windows over 63 columns, a profile LENG other than the library's, a profile whose row
+ * count is not LENG or that numbers a row twice, a row with fewer than 20 values, a negative, infinite or NaN PRIOR, and
+ * a value v whose probability 2^(-v/1000) is 0 or infinite in double -- '*' among them: the reference reads it as log 0,
+ * and 0 * log 0 makes every column whose window holds a zero count NaN.  Non-finite window weights are refused too.
+ * hhg_crf_create refuses the text of a context library, and this call the text of a CRF. */
+int hhg_context_library_create(hhg_ctx* ctx, const char* text, int64_t len, double weight_center, double weight_decay,
+                               hhg_crf** out);
+int hhg_context_library_parse_host(const char* text, int64_t len, double weight_center, double weight_decay, hhg_crf** out);
 /* Host only: LENG and whether the record carries an ss_pred sequence (no numbers are parsed). */
 int hhg_hhm_scan(const char* rec, int64_t len, int32_t* L, int32_t* has_ss);
 /* Host only: the tokeniser hhg_db_create_hhm runs per record, exposed for inspection and CPU-side tests.
