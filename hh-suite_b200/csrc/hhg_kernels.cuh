@@ -452,17 +452,36 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
       }
       dtMM = tMM; dtDG = tDG; dtGD = tGD; dtIM = tIM;
 
-      // running maximum, :423-455: ONE test per column on the maximum of the R new MM values (a tree of
-      // FMNMX, 1 instruction per row instead of compare+branch per cell); only when it can matter the
-      // rows are examined in ascending order.  Strips are swept column-major, the reference row-major:
-      // on an exact tie the earlier ROW must win (mm == best && i < bi).
+      // running maximum, :423-455: ONE test per column on the maximum m of the R new MM values (a tree of
+      // FMNMX, 1 instruction per row instead of compare+branch per cell).  Strips are swept column-major, the
+      // reference row-major: on an exact tie the earlier ROW must win (mm == best && i < bi).
       {
         float c0 = MM[0], c1 = MM[1], c2 = MM[2], c3 = MM[3];   // four interleaved chains (R is a multiple of 4)
 #pragma unroll
         for (int r = 4; r < R; r += 4) {
           c0 = fmaxf(c0, MM[r]); c1 = fmaxf(c1, MM[r + 1]); c2 = fmaxf(c2, MM[r + 2]); c3 = fmaxf(c3, MM[r + 3]);
         }
-        if (fmaxf(fmaxf(c0, c1), fmaxf(c2, c3)) >= bc) {
+        const float m = fmaxf(fmaxf(c0, c1), fmaxf(c2, c3));
+        if (LOCAL) {
+          // every row up to Lq is a candidate: the column's record is its argmax, the FIRST row that reaches the
+          // maximum, taken when it beats the strip's best or ties it at a smaller row.  A warp vote skips the select
+          // chain on columns where no lane can move; the chain and the update are predicated, with no per-row branch.
+          // The maximum's bits are the row's: MM is never -0 (its last FADD adds Si, which is never -0).
+          if (__any_sync(0xffffffffu, m >= bcmp)) {
+            float mc = m;
+            if (i0 + R > Lq) {   // the last strip of a query that is not a multiple of R: rows past Lq do not count
+              mc = -INFINITY;
+#pragma unroll
+              for (int r = 0; r < R; ++r) mc = fmaxf(mc, (i0 + 1 + r <= Lq) ? MM[r] : -INFINITY);
+            }
+            int r1 = R - 1;
+#pragma unroll
+            for (int r = R - 2; r >= 0; --r) r1 = (MM[r] == mc) ? r : r1;
+            const int i = i0 + 1 + r1;
+            if (mc >= bcmp && (mc > best || i < bi)) { best = mc; bi = i; bj = j; }
+          }
+        } else if (m >= bc) {
+          // global mode, where only row Lq and column Lt count: rows in ascending order
 #pragma unroll
           for (int r = 0; r < R; ++r) {
             const float mm = MM[r];
