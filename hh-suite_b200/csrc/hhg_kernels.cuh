@@ -222,6 +222,17 @@ constexpr size_t kRingBytes = 2 * kJcSlot * 16;   // 7168 B per warp
 
 #define HHG_NEG (-FLT_MAX)
 
+// x with -0 replaced by +0 (x + +0 under round-to-nearest); every other value unchanged
+__device__ __forceinline__ float pos_zero(float x) { return __fadd_rn(x, 0.0f); }
+
+// the sign bits of a (row r) and b (row r+1) as 0x00 / 0xFF bytes: selector nibble 0xB (0xF) puts the replicated msb
+// of byte 3 of a (of b) in its byte.  Inline PTX because __byte_perm drops the replicate bit of a selector nibble
+__device__ __forceinline__ uint32_t sign_bytes(float a, float b, uint32_t sel) {
+  uint32_t p;
+  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(p) : "r"(__float_as_uint(a)), "r"(__float_as_uint(b)), "r"(sel));
+  return p;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Forward pass.  R rows per strip (multiple of 4).  LOCAL: par.loc.  SS: PRED_PRED ss term.
 // CELLOFF: cell-off bit input (alternative alignments / excluded regions).
@@ -298,14 +309,16 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
     //     (up), and both add q_m2m(r+1) first; Y[r] = MI(r-1, j-1) + q_m2m(r) is that shared sum.
     //   * the other diagonal reads (c1..c4 of row r+1) take partial sums that row r forms from its old values
     //     before it overwrites them (pMM, pGD, pIM, pDG).
+    // The gap-state flags read sign bits and need every DP value to differ from -0 (see the row body).  -i·egq and
+    // -j·egt are -0 when a gap cost is 0, so the boundary values take +0 for -0 (pos_zero).
     float MM[R], GD[R], IM[R], DG[R], Y[R];
 #pragma unroll
     for (int r = 0; r < R; ++r) {
-      MM[r] = __fmul_rn((float)(-(i0 + 1 + r)), P.egq);
+      MM[r] = pos_zero(__fmul_rn((float)(-(i0 + 1 + r)), P.egq));
       GD[r] = IM[r] = DG[r] = HHG_NEG;
     }
     // boundary row i0 at column j-1 (diagonal of the strip's first row)
-    float dtMM = __fmul_rn((float)(-i0), P.egq), dtDG = HHG_NEG, dtGD = HHG_NEG, dtIM = HHG_NEG;
+    float dtMM = pos_zero(__fmul_rn((float)(-i0), P.egq)), dtDG = HHG_NEG, dtGD = HHG_NEG, dtIM = HHG_NEG;
 
     float best = HHG_NEG;
     int bi = 0, bj = 0;
@@ -346,7 +359,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
       // tag is there, then prefetch column j+1
       float tMM, tDG, tMI, tGD, tIM;
       if (s == 0) {
-        tMM = __fmul_rn((float)(-j), P.egt);   // :148
+        tMM = pos_zero(__fmul_rn((float)(-j), P.egt));   // :148
         tDG = tMI = tGD = tIM = HHG_NEG;
       } else {
         // all five words must carry the producer's tag.  One warp vote on the common path; strip s-1 normally runs
@@ -371,8 +384,12 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
       const float bcmp = (j <= Lt) ? best : INFINITY;   // padded columns never become the maximum
       float bc = bcmp;
 
+      // The trace word of 4 rows starts at 6 in every byte and takes each row's MM code XOR 6 by XOR (see b below).
       // (t_ss & P.zero) is 0; it only keeps the 4th register of the operand LDS.128 live (see ld_slot)
-      uint32_t word = SS ? 0u : (t_ss & P.zero);
+      constexpr uint32_t kWord0 = 0x06060606u;
+      uint32_t word = kWord0 ^ (SS ? 0u : (t_ss & P.zero));
+      uint32_t eb = 0u;                                     // b of the pair's even row
+      float eGD = 0.f, eIM = 0.f, eDG = 0.f, eMI = 0.f;   // and its gap-flag differences
 #pragma unroll
       for (int r = 0; r < R; ++r) {
         float4 q[5];
@@ -380,8 +397,11 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
         for (int k = 0; k < 5; ++k) q[k] = qs[r * 7 + k];
         const float q_m2m = qa.x, q_m2d = qa.y, q_d2m = qa.z, q_d2d = qa.w;
         const float q_i2m = qb.x, q_i2i = qb.y, q_m2i = qb.z;
+        const uint32_t q_ss = __float_as_uint(qb.w);
+        const int sh = 8 * (r & 3);   // this row's byte of the trace word
 
-        // 5-way maximum with the reference's strict-'>' / first-wins rule, :241-273
+        // 5-way maximum with the reference's strict-'>' / first-wins rule, :241-273.  b is the MM code XOR 6, already
+        // in this row's byte: code 6 (MI) becomes 0, so every select of the chain has one constant and no MOV
         uint32_t b;
         float mm;
         const float c1 = __fadd_rn(pMM, t_m2m);     // (MM(i-1,j-1) + q_m2m) + t_m2m
@@ -395,39 +415,51 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
         mm = fmaxf(fmaxf(smin, c1), c2);
         mm = fmaxf(fmaxf(mm, c3), c4);
         mm = fmaxf(mm, c5);
-        b = 6u;
-        b = (c4 == mm) ? 5u : b;
-        b = (c3 == mm) ? 4u : b;
-        b = (c2 == mm) ? 3u : b;
-        b = (c1 == mm) ? 2u : b;
-        b = (smin == mm) ? 0u : b;
+        b = (c4 == mm) ? (5u ^ 6u) << sh : 0u;
+        b = (c3 == mm) ? (4u ^ 6u) << sh : b;
+        b = (c2 == mm) ? (3u ^ 6u) << sh : b;
+        b = (c1 == mm) ? (2u ^ 6u) << sh : b;
+        b = (smin == mm) ? (0u ^ 6u) << sh : b;
 #else
-        b = (c1 > smin) ? 2u : 0u; mm = fmaxf(smin, c1);
-        b = (c2 > mm) ? 3u : b;    mm = fmaxf(mm, c2);
-        b = (c3 > mm) ? 4u : b;    mm = fmaxf(mm, c3);
-        b = (c4 > mm) ? 5u : b;    mm = fmaxf(mm, c4);
-        b = (c5 > mm) ? 6u : b;    mm = fmaxf(mm, c5);
+        b = (c1 > smin) ? (2u ^ 6u) << sh : 6u << sh; mm = fmaxf(smin, c1);
+        b = (c2 > mm) ? (3u ^ 6u) << sh : b;          mm = fmaxf(mm, c2);
+        b = (c3 > mm) ? (4u ^ 6u) << sh : b;          mm = fmaxf(mm, c3);
+        b = (c4 > mm) ? (5u ^ 6u) << sh : b;          mm = fmaxf(mm, c4);
+        b = (c5 > mm) ? 0u : b;                       mm = fmaxf(mm, c5);
 #endif
 
         float Si = log2f4_dev(dot20_dev(tp, q));                     // :277
         if (SS) {
-          const uint32_t q_ss = __float_as_uint(qb.w);
           Si = __fadd_rn(__fmul_rn(P.ssw, s33[q_ss * 44 + t_ss]), Si);   // :210,279
         }
         Si = __fadd_rn(Si, P.shift);                                   // :281
         mm = __fadd_rn(mm, Si);
 
         const float oMM = MM[r], oGD = GD[r], oIM = IM[r], oDG = DG[r];   // (i, j-1)
-        float a1, a2, gd, im, dg, mi;
+        // the next row's diagonal partial sums, from this row's old values and before its new ones: with no old value
+        // live past its replacement ptxas keeps each state in one register (otherwise ~40 copies per column)
+        if (r + 1 < R) {
+          qa = qs[(r + 1) * 7 + 5]; qb = qs[(r + 1) * 7 + 6];
+          pMM = __fadd_rn(oMM, qa.x); pGD = __fadd_rn(oGD, qa.x); pIM = __fadd_rn(oIM, qb.x);
+          pDG = __fadd_rn(oDG, qa.z);
+        }
+        // Gap-state flags.  The reference's a1 > a2 is the sign bit of a2 - a1 (an FADD instead of a compare and a
+        // select on the integer pipe): a difference of two floats is 0 only when they are equal, overflow and
+        // underflow keep the sign, and the canonical NaN of -inf - -inf or inf - inf has a clear sign bit, as a1 > a2
+        // is false there.  The one exception, (-0) - (+0) = -0, cannot occur: under round-to-nearest a sum is -0 only
+        // when both addends are -0, every sum here and in the MM recurrence has an addend that is a DP value, Si or
+        // -FLT_MAX, and so by induction no DP value is -0 once the boundary values are not (pos_zero above).  Si is
+        // never -0: log2f4's e is an exact difference, +0 when it vanishes.  Transitions may be -0.
+        float a1, a2, gd, im, dg, mi, dGD, dIM, dDG, dMI;
         a1 = __fadd_rn(oMM, t_m2d); a2 = __fadd_rn(oGD, t_d2d);                                // :307
-        b |= (a1 > a2) ? 8u : 0u;  gd = fmaxf(a1, a2);
+        dGD = __fsub_rn(a2, a1); gd = fmaxf(a1, a2);
         a1 = __fadd_rn(__fadd_rn(oMM, q_m2i), t_m2m); a2 = __fadd_rn(__fadd_rn(oIM, q_i2i), t_m2m);   // :324
-        b |= (a1 > a2) ? 16u : 0u; im = fmaxf(a1, a2);
+        dIM = __fsub_rn(a2, a1); im = fmaxf(a1, a2);
         a1 = __fadd_rn(uMM, q_m2d); a2 = __fadd_rn(uDG, q_d2d);                                // :340
-        b |= (a1 > a2) ? 32u : 0u; dg = fmaxf(a1, a2);
+        dDG = __fsub_rn(a2, a1); dg = fmaxf(a1, a2);
         Y[r] = __fadd_rn(uMI, q_m2m);                                                           // c5 of column j+1
         a1 = __fadd_rn(__fadd_rn(uMM, q_m2m), t_m2i); a2 = __fadd_rn(Y[r], t_i2i);             // :358
-        b |= (a1 > a2) ? 64u : 0u; mi = fmaxf(a1, a2);
+        dMI = __fsub_rn(a2, a1); mi = fmaxf(a1, a2);
 
         if (CELLOFF) {                                                 // :373-392
           const float off = ((cow >> r) & 1u) ? HHG_NEG : 0.0f;
@@ -435,16 +467,21 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, (R <= 12) ? 3 : 2)   // reg
           dg = __fadd_rn(dg, off); mi = __fadd_rn(mi, off);
         }
 
-        word |= b << (8 * (r & 3));
+        // rows r-1 and r go into their bytes together: one LOP3 for both MM codes, and per flag one PRMT and one LOP3
+        if (r & 1) {
+          const int q = r & 2;   // byte of row r-1
+          const uint32_t sel = 0xFBu << (4 * q);
+          word ^= eb ^ b;
+          word |= sign_bytes(eGD, dGD, sel) & (0x0808u << (8 * q));
+          word |= sign_bytes(eIM, dIM, sel) & (0x1010u << (8 * q));
+          word |= sign_bytes(eDG, dDG, sel) & (0x2020u << (8 * q));
+          word |= sign_bytes(eMI, dMI, sel) & (0x4040u << (8 * q));
+        } else {
+          eb = b; eGD = dGD; eIM = dIM; eDG = dDG; eMI = dMI;
+        }
         if ((r & 3) == 3) {
           __stcs(btc + (size_t)(r >> 2) * bt_row_stride, word);
-          word = 0;
-        }
-        // the next row's diagonal partial sums, from this row's old values before they are overwritten
-        if (r + 1 < R) {
-          qa = qs[(r + 1) * 7 + 5]; qb = qs[(r + 1) * 7 + 6];
-          pMM = __fadd_rn(oMM, qa.x); pGD = __fadd_rn(oGD, qa.x); pIM = __fadd_rn(oIM, qb.x);
-          pDG = __fadd_rn(oDG, qa.z);
+          word = kWord0;
         }
         // this row's new values are the next row's up
         uMM = mm; uDG = dg; uMI = mi;

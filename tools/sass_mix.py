@@ -5,7 +5,10 @@ usage: python tools/sass_mix.py [--compile] [--lib PATH] [--all] [--filter SUBST
 For every k_viterbi<R,LOCAL,SS,CELLOFF> instantiation in the library it finds the column loop (see column_loop)
 and prints its static instructions per row visit (one row of one column for the 32 lanes of a warp) by opcode, the
 MOVs, LDS (query rows and operand ring) and LDGSTS (cp.async into the ring) per column, registers, the size of the running-maximum rare path inside the loop and, with --compile, the
-spill bytes ptxas reports.  --compile builds the library with the flags of build.py into a
+spill bytes ptxas reports.  It also splits the instructions per row visit between the FP32 pipe and the ALU pipe
+(PIPES below), and sums the stall counts ptxas encodes in each instruction's control bits over one pass of the loop
+(cycles per column before latency and dependency waits), with how many instructions stall for 2 cycles, the count
+ptxas gives back-to-back ALU-pipe instructions, which issue at half the FP32 rate.  --compile builds the library with the flags of build.py into a
 temporary directory; otherwise --lib (default hh-suite_b200/libhhg.so) is read.
 """
 from __future__ import annotations
@@ -25,6 +28,10 @@ import build  # noqa: E402
 CUDA_BIN = os.path.dirname(build.NVCC)
 MANGLED = re.compile(r"_ZN3hhg9k_viterbiILi(\d+)ELb(\d)ELb(\d)ELb(\d)EEEvNS_9VitParamsE")
 INSN = re.compile(r"/\*([0-9a-f]{4,})\*/\s+(@!?U?P\w+\s+)?([A-Z][A-Z0-9_]*)([^;]*);")
+HEX = re.compile(r"/\*\s*0x([0-9a-f]{16})\s*\*/\s*$")
+# the pipe each opcode issues to on sm_90 (the rest: memory, moves, branches, uniform datapath)
+PIPES = {"FP32": {"FADD", "FMUL", "FFMA", "IMAD", "HFMA2"},
+         "ALU": {"FMNMX", "FSETP", "FSEL", "SEL", "ISETP", "IADD3", "LOP3", "LEA", "SHF", "PRMT", "PLOP3", "IMNMX"}}
 
 
 def name_of(m: re.Match) -> str:
@@ -47,22 +54,31 @@ def compile_lib(tmp: str) -> tuple[str, dict]:
     return out, spills
 
 
-def functions(lib: str) -> dict[str, list[tuple[int, str, str]]]:
+def functions(lib: str) -> tuple[dict[str, list[tuple[int, str, str]]], dict[str, dict[int, int]]]:
+    """Per instantiation its instructions (address, opcode, operands) and the stall count of each address: bits 41-44
+    of the second 64-bit word of the 128-bit encoding, which cuobjdump prints on the line after the instruction."""
     sass = subprocess.run([os.path.join(CUDA_BIN, "cuobjdump"), "-sass", lib], capture_output=True, text=True,
                           check=True).stdout
-    funcs, cur = {}, None
+    funcs, stalls, cur, last = {}, {}, None, None
     for line in sass.splitlines():
         if "Function :" in line:
             m = MANGLED.search(line)
             cur = name_of(m) if m else None
             if cur:
-                funcs[cur] = []
+                funcs[cur], stalls[cur] = [], {}
+            last = None
             continue
         if cur:
             m = INSN.search(line)
             if m:
-                funcs[cur].append((int(m.group(1), 16), m.group(3), m.group(4)))
-    return funcs
+                last = int(m.group(1), 16)
+                funcs[cur].append((last, m.group(3), m.group(4)))
+            elif last is not None:
+                h = HEX.search(line)
+                if h:
+                    stalls[cur][last] = (int(h.group(1), 16) >> 41) & 0xF
+                last = None
+    return funcs, stalls
 
 
 def registers(lib: str) -> dict[str, tuple[int, int]]:
@@ -118,7 +134,7 @@ def main() -> None:
         lib = args.lib
         if args.compile:
             lib, spills = compile_lib(tmp)
-        funcs = functions(lib)
+        funcs, stalls = functions(lib)
         regs = registers(lib)
     names = sorted(funcs, key=lambda n: [int(x) for x in re.findall(r"\d+", n)], reverse=True)
     if not args.all:
@@ -141,6 +157,11 @@ def main() -> None:
               f"MOV {mix['MOV']}, LDS {mix['LDS']}, LDGSTS {mix['LDGSTS']} per column; {reg} registers, stack {stack} B"
               + (f", spill stores {sp[0]} B / loads {sp[1]} B" if sp else "")
               + f"; widest skipped block {cold} ({(len(loop) - cold) / R:.1f} per row visit without it)")
+        pipe = {k: sum(c for op, c in mix.items() if op in v) for k, v in PIPES.items()}
+        st = [stalls[n][a] for a, _, _ in loop]
+        print(f"   per row visit: FP32 pipe {pipe['FP32'] / R:.1f}, ALU pipe {pipe['ALU'] / R:.1f}, other "
+              f"{(len(loop) - sum(pipe.values())) / R:.1f}; ptxas stall cycles {sum(st)} per column, "
+              f"{st.count(2)} instructions with stall 2")
         print("   " + "  ".join(f"{op} {c / R:.2f}" for op, c in mix.most_common()))
 
 
