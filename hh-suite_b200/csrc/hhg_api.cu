@@ -134,6 +134,7 @@ struct hhg_ctx {
   std::vector<float> h_q_pav;
   bool has_q_pav = false;
   DevBuf<float> d_q_pav, d_pb;
+  float h_pb[20] = {};   // host copy of d_pb (the background of columnscore 0 in the last batch search)
   // excluded regions (-excl / -template_excl), applied to every search until cleared: ex = {q_lo[ex_nq], q_hi[ex_nq],
   // t_lo[ex_nt], t_hi[ex_nt]} as k_celloff_regions and k_mac_realign read it from d_ex
   std::vector<int> ex;
@@ -208,6 +209,7 @@ struct Wave {
 };
 
 struct hhg_plan {
+  bool built = false;   // false after a failed (re)build: the host tables no longer describe the device buffers
   const hhg_db* db = nullptr;
   unsigned long long db_serial = 0;
   int device = 0;
@@ -228,6 +230,7 @@ struct hhg_plan {
   int nm_mode = -1;                       // >= 0: columnscore of the null model fused into the stream (raw shard)
   int jc_nm_mode = -2;                    // nm_mode / query batch the stream was built with
   unsigned long long jc_query_serial = 0;
+  float jc_pb[20] = {};                   // pb the stream was divided by (nm_mode 0)
   std::vector<Wave> waves;
   long long path_total = 0;
   // device
@@ -1495,7 +1498,7 @@ static int plan_build(hhg_ctx* ctx, hhg_plan* pl, const hhg_db* db, int n, const
   const int R = plan_strip_rows(ctx, req_query, n);
   // the common case of a repeated request (same shard, same target list, same query batch geometry, e.g. every
   // query of a series against the whole shard) reuses the plan: no host sort, no uploads
-  if (pl->db == db && pl->db_serial == db->serial && pl->n == n && pl->R == R && pl->q_L == ctx->q_L &&
+  if (pl->built && pl->db == db && pl->db_serial == db->serial && pl->n == n && pl->R == R && pl->q_L == ctx->q_L &&
       pl->q_row0 == ctx->q_row0 && !pl->ids.empty() && pl->max_bt_bytes == ctx->max_bt_bytes) {
     bool same = true;
     if (ids) same = memcmp(ids, pl->ids.data(), (size_t)n * 4) == 0;
@@ -1506,6 +1509,8 @@ static int plan_build(hhg_ctx* ctx, hhg_plan* pl, const hhg_db* db, int n, const
     }
     if (same) { pl->celloff = false; return HHG_OK; }
   }
+  // any early return below leaves the plan half rewritten: it must neither be reused nor run until a build succeeds
+  pl->built = false;
   pl->db = db;
   pl->db_serial = db->serial;
   pl->device = db->device;
@@ -1637,6 +1642,7 @@ static int plan_build(hhg_ctx* ctx, hhg_plan* pl, const hhg_db* db, int n, const
   CK(H2D(pl->d_job_target.p, job_target.data(), job_target.size() * 4));
   CK(H2D(pl->d_items.p, pl->items.data(), pl->items.size() * sizeof(int2)));
   CK(cudaStreamSynchronize(st));
+  pl->built = true;
   return HHG_OK;
 }
 
@@ -1759,6 +1765,7 @@ static int launch_viterbi(hhg_ctx* ctx, const VitParams& P, bool local, bool ss,
 
 static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
   if (!ctx || !pl) return fail(HHG_EINVAL, "hhg_plan_run: bad argument");
+  if (!pl->built) return fail(HHG_EINVAL, "hhg_plan_run: the plan's last build failed");
   if (pl->q_L != ctx->q_L || pl->q_row0 != ctx->q_row0) return fail(HHG_EINVAL, "plan was made for another query (batch) geometry");
   const hhg_db* db = pl->db;
   const bool fused = pl->nm_mode >= 0;     // null model factored in per job while the operand stream is built
@@ -1779,9 +1786,11 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
   }
   CK(cudaMemsetAsync(pl->d_counter.p, 0, pl->waves.size() * 4, st));
   if (pl->jc_version != db->cols_version || pl->jc_nm_mode != pl->nm_mode ||
-      (fused && pl->jc_query_serial != ctx->query_serial)) {
+      (fused && pl->jc_query_serial != ctx->query_serial) ||
+      (pl->nm_mode == 0 && memcmp(pl->jc_pb, ctx->h_pb, sizeof pl->jc_pb) != 0)) {
     // (re)build the job-interleaved operand stream: once per plan, again after every hhg_db_apply_null_model (the
-    // prepared emissions changed) and, with the fused null model, for every new query batch
+    // prepared emissions changed) and, with the fused null model, for every new query batch and, with columnscore 0,
+    // for every new pb (k_backtrace divides by the current one, so the forward pass must too)
     int maxL = 0;
     for (const JobDesc& jd : pl->jobs) maxL = std::max(maxL, jd.Lmax);
     dim3 grid((unsigned)pl->njobs, (unsigned)std::min(64, (maxL + 7) / 8), 1);
@@ -1793,6 +1802,7 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
     pl->jc_version = db->cols_version;
     pl->jc_nm_mode = pl->nm_mode;
     pl->jc_query_serial = ctx->query_serial;
+    memcpy(pl->jc_pb, ctx->h_pb, sizeof pl->jc_pb);
   }
   for (size_t wi = 0; wi < pl->waves.size(); ++wi) {
     const Wave& w = pl->waves[wi];
@@ -1900,6 +1910,7 @@ hhg_plan* hhg_ctx_last_plan(hhg_ctx* ctx) { return ctx ? ctx->scratch_plan : nul
 
 int hhg_plan_debug_bt(hhg_ctx* ctx, hhg_plan* pl, int k, uint8_t* bt) {
   if (!ctx || !pl || !bt || k < 0 || k >= pl->n) return fail(HHG_EINVAL, "hhg_plan_debug_bt: bad argument");
+  if (!pl->built) return fail(HHG_EINVAL, "hhg_plan_debug_bt: the plan's last build failed");
   if (pl->waves.size() != 1) return fail(HHG_EINVAL, "debug_bt needs a single-wave plan");
   CK(cudaSetDevice(ctx->device));
   const ReqDesc& rq = pl->reqs[k];
@@ -1957,10 +1968,10 @@ int hhg_viterbi_search_batch(hhg_ctx* ctx, const hhg_db* db, int n, const int32_
     if (columnscore < 0 || columnscore > 3) return fail(HHG_EINVAL, "hhg_viterbi_search_batch: columnscore %d", columnscore);
     if (!ctx->has_q_pav) return fail(HHG_EINVAL, "hhg_viterbi_search_batch: raw shard needs q_pav in hhg_query_set_batch");
     if (columnscore == 0 && !pb) return fail(HHG_EINVAL, "hhg_viterbi_search_batch: columnscore 0 needs pb");
-    float h[20] = {0};
-    if (pb) memcpy(h, pb, 80);
+    memset(ctx->h_pb, 0, sizeof ctx->h_pb);
+    if (pb) memcpy(ctx->h_pb, pb, sizeof ctx->h_pb);
     CK(ctx->d_pb.ensure(20));
-    CK(cudaMemcpyAsync(ctx->d_pb.p, h, 80, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_pb.p, ctx->h_pb, sizeof ctx->h_pb, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     pl->nm_mode = columnscore;
   }
