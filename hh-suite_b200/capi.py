@@ -37,6 +37,7 @@ SYMBOLS = ["hhg_last_error", "hhg_ctx_create", "hhg_ctx_destroy", "hhg_ctx_sync"
            "hhg_plan_cells", "hhg_plan_padded_cells", "hhg_plan_algorithmic_bytes", "hhg_plan_debug_bt",
            "hhg_csdb_create", "hhg_csdb_destroy", "hhg_prefilter_ungapped", "hhg_prefilter_ungapped_run",
            "hhg_prefilter_fetch", "hhg_prefilter_select", "hhg_log2lin", "hhg_mac_query_set", "hhg_mac_realign",
+           "hhg_mac_query_set_batch", "hhg_mac_realign_batch",
            "hhg_mac_debug_posterior", "hhg_prefilter_build_profile", "hhg_prefilter_corrected_score",
            "hhg_prefilter_sw", "hhg_prefilter_evalue", "hhg_prefilter_corrected_scores", "hhg_prefilter_evalues",
            "hhg_comm_unique_id", "hhg_comm_create", "hhg_comm_destroy", "hhg_comm_rank", "hhg_comm_world",
@@ -267,6 +268,10 @@ def load():
     L.hhg_mac_realign.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, c_i32p, c_i64p, c_i32p, c_i32p, c_i64p,
                                   c_i32p, c_i32p, C.POINTER(MacParams), C.c_void_p, c_i32p, c_i32p, c_u8p, c_f32p,
                                   C.c_size_t]
+    L.hhg_mac_query_set_batch.argtypes = [C.c_void_p, C.c_int, c_i32p, C.c_void_p, C.c_void_p, c_f32p]
+    L.hhg_mac_realign_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, c_i32p, c_i32p, c_i64p, c_i32p, c_i32p,
+                                        c_i64p, c_i32p, c_i32p, C.c_int, c_f32p, C.POINTER(MacParams), C.c_void_p,
+                                        c_i32p, c_i32p, c_u8p, c_f32p, C.c_size_t]
     L.hhg_mac_debug_posterior.argtypes = [C.c_void_p, C.c_int, c_f32p]
     L.hhg_prefilter_fetch.argtypes = [C.c_void_p, C.c_void_p, c_i32p]
     L.hhg_prefilter_build_profile.argtypes = [C.c_int, c_f32p, c_f32p, c_f32p, C.c_int, C.c_int, c_u8p]
@@ -332,7 +337,7 @@ def load():
     L.hhg_query_set_batch.argtypes = [C.c_void_p, C.c_int, c_i32p, C.c_void_p, C.c_void_p, C.c_void_p, c_f32p, c_f32p,
                                       C.POINTER(Params)]
     L.hhg_viterbi_search_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, c_i32p, C.c_int, c_f32p, C.c_void_p,
-                                           c_u8p, C.c_size_t]
+                                           c_u8p, C.c_size_t, c_i64p, c_i32p, c_i32p]
     L.hhg_plan_topk_paths.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, c_u8p]
     L.hhg_ctx_last_plan.argtypes = [C.c_void_p]
     L.hhg_ctx_last_plan.restype = C.c_void_p
@@ -406,14 +411,29 @@ def mac_query_set(ctx, q_p, q_tr_lin):
     assert q_tr_lin.shape == (Lq + 1, 7)
     _ck(ctx.L.hhg_mac_query_set(ctx.h, Lq, _p(q_p, c_f32p), _p(q_tr_lin, c_f32p)))
     ctx.mac_Lq = Lq
+    ctx.mac_batch_Lq = np.array([Lq], np.int32)
 
 
-def mac_realign(ctx, db, targets, vits, excl=None, local=True, shift=-0.03, mact=0.35):
-    """PosteriorDecoder::realign for a batch of hits.  vits[r] = (i1, i2, j1, j2, nsteps, i_steps, j_steps) with
-    1-based step arrays (Hit.i / Hit.j); excl[r] = (alt_i, alt_j) of earlier MAC alignments of that template or None.
-    Returns (hits[MAC_HIT_DTYPE], list of dict(i, j, states, P_posterior) with 1-based step arrays)."""
-    n = len(targets)
-    targets = np.ascontiguousarray(targets, np.int32)
+def mac_query_set_batch(ctx, queries, q_pav=None):
+    """Queries for hhg_mac_realign_batch: queries = list of (HMM::p, LINEAR transitions); q_pav [nq, 20] (HMM::pav of
+    each query) for realignments over a raw shard."""
+    nq = len(queries)
+    ps = [np.ascontiguousarray(q[0], np.float32) for q in queries]
+    trs = [np.ascontiguousarray(q[1], np.float32) for q in queries]
+    Lq = np.array([p.shape[0] - 2 for p in ps], np.int32)
+    for L, t in zip(Lq, trs):
+        assert t.shape == (L + 1, 7)
+    pp = (C.c_void_p * nq)(*[p.ctypes.data for p in ps])
+    tp = (C.c_void_p * nq)(*[t.ctypes.data for t in trs])
+    qv = None if q_pav is None else np.ascontiguousarray(q_pav, np.float32)
+    _ck(ctx.L.hhg_mac_query_set_batch(ctx.h, nq, _p(Lq, c_i32p), pp, tp, _p(qv, c_f32p)))
+    ctx.mac_Lq = int(Lq[0])
+    ctx.mac_batch_Lq = Lq
+
+
+def _mac_inputs(vits, excl):
+    """vit[n,5], vit_off, vit_i, vit_j and (excl_off, excl_i, excl_j) or Nones, as hhg_mac_realign(_batch) takes them."""
+    n = len(vits)
     vit = np.zeros((n, 5), np.int32)
     voff = np.zeros(n + 1, np.int64)
     for r, v in enumerate(vits):
@@ -433,6 +453,26 @@ def mac_realign(ctx, db, targets, vits, excl=None, local=True, shift=-0.03, mact
         for r, e in enumerate(excl):
             if e is not None and len(e[0]):
                 ei[eoff[r]:eoff[r + 1]] = e[0]; ej[eoff[r]:eoff[r + 1]] = e[1]
+    return vit, voff, vi, vj, eoff, ei, ej
+
+
+def _mac_paths(hits, oi, oj, os_, op):
+    """Per request: dict(i, j, states, P_posterior) with 1-based step arrays, sliced from the output buffers."""
+    paths = []
+    for r in range(len(hits)):
+        o, ns = int(hits["path_off"][r]), int(hits["nsteps"][r])
+        paths.append(dict(i=oi[o:o + ns + 1].copy(), j=oj[o:o + ns + 1].copy(), states=os_[o:o + ns + 1].copy(),
+                          P_posterior=op[o:o + ns + 1].copy()))
+    return paths
+
+
+def mac_realign(ctx, db, targets, vits, excl=None, local=True, shift=-0.03, mact=0.35):
+    """PosteriorDecoder::realign for a batch of hits.  vits[r] = (i1, i2, j1, j2, nsteps, i_steps, j_steps) with
+    1-based step arrays (Hit.i / Hit.j); excl[r] = (alt_i, alt_j) of earlier MAC alignments of that template or None.
+    Returns (hits[MAC_HIT_DTYPE], list of dict(i, j, states, P_posterior) with 1-based step arrays)."""
+    n = len(targets)
+    targets = np.ascontiguousarray(targets, np.int32)
+    vit, voff, vi, vj, eoff, ei, ej = _mac_inputs(vits, excl)
     cap = int(np.sum(ctx.mac_Lq + db.Lh[np.clip(targets, 0, db.n - 1)].astype(np.int64) + 2))
     hits = np.zeros(n, MAC_HIT_DTYPE)
     oi = np.zeros(cap, np.int32); oj = np.zeros(cap, np.int32); os_ = np.zeros(cap, np.uint8); op = np.zeros(cap, np.float32)
@@ -441,12 +481,29 @@ def mac_realign(ctx, db, targets, vits, excl=None, local=True, shift=-0.03, mact
                               _p(vj, c_i32p), _p(eoff, c_i64p), _p(ei, c_i32p), _p(ej, c_i32p), C.byref(pp),
                               hits.ctypes.data_as(C.c_void_p), _p(oi, c_i32p), _p(oj, c_i32p), _p(os_, c_u8p),
                               _p(op, c_f32p), cap))
-    paths = []
-    for r in range(n):
-        o, ns = int(hits["path_off"][r]), int(hits["nsteps"][r])
-        paths.append(dict(i=oi[o:o + ns + 1].copy(), j=oj[o:o + ns + 1].copy(), states=os_[o:o + ns + 1].copy(),
-                          P_posterior=op[o:o + ns + 1].copy()))
-    return hits, paths
+    return hits, _mac_paths(hits, oi, oj, os_, op)
+
+
+def mac_realign_batch(ctx, db, req_query, targets, vits, excl=None, columnscore=1, pb=None, local=True, shift=-0.03,
+                      mact=0.35):
+    """hhg_mac_realign_batch: request r realigns query req_query[r] of the last mac_query_set_batch against
+    targets[r]; vits / excl and the result as in mac_realign.  columnscore / pb: the null model of a raw shard."""
+    n = len(targets)
+    rq = np.ascontiguousarray(req_query, np.int32); targets = np.ascontiguousarray(targets, np.int32)
+    vit, voff, vi, vj, eoff, ei, ej = _mac_inputs(vits, excl)
+    qL = ctx.mac_batch_Lq
+    cap = int(np.sum(qL[np.clip(rq, 0, len(qL) - 1)].astype(np.int64) +
+                     db.Lh[np.clip(targets, 0, db.n - 1)].astype(np.int64) + 2))
+    hits = np.zeros(n, MAC_HIT_DTYPE)
+    oi = np.zeros(cap, np.int32); oj = np.zeros(cap, np.int32); os_ = np.zeros(cap, np.uint8); op = np.zeros(cap, np.float32)
+    pp = MacParams(1 if local else 0, shift, mact)
+    pbv = None if pb is None else np.ascontiguousarray(pb, np.float32)
+    _ck(ctx.L.hhg_mac_realign_batch(ctx.h, db.h, n, _p(rq, c_i32p), _p(targets, c_i32p), _p(vit, c_i32p),
+                                    _p(voff, c_i64p), _p(vi, c_i32p), _p(vj, c_i32p), _p(eoff, c_i64p), _p(ei, c_i32p),
+                                    _p(ej, c_i32p), columnscore, _p(pbv, c_f32p), C.byref(pp),
+                                    hits.ctypes.data_as(C.c_void_p), _p(oi, c_i32p), _p(oj, c_i32p), _p(os_, c_u8p),
+                                    _p(op, c_f32p), cap))
+    return hits, _mac_paths(hits, oi, oj, os_, op)
 
 
 def mac_debug_posterior(ctx, request, Lt):
@@ -863,6 +920,21 @@ class Plan:
             self.h = None
 
 
+def _exclusions(exclusions):
+    """(excl_off, excl_i, excl_j) of a per-request list of (i_steps, j_steps) or None entries; Nones without a list."""
+    if exclusions is None:
+        return None, None, None
+    cnt = np.array([0 if e is None else len(e[0]) for e in exclusions], np.int64)
+    eo = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int64)
+    ei = np.concatenate([np.asarray(e[0], np.int32) for e in exclusions if e is not None] or
+                        [np.zeros(0, np.int32)]).astype(np.int32)
+    ej = np.concatenate([np.asarray(e[1], np.int32) for e in exclusions if e is not None] or
+                        [np.zeros(0, np.int32)]).astype(np.int32)
+    if len(ei) == 0:
+        ei = np.zeros(1, np.int32); ej = np.zeros(1, np.int32)
+    return eo, ei, ej
+
+
 def viterbi_search(ctx: Context, db: TargetDB, ids=None, exclusions=None, want_paths=True, hits=None,
                    paths=None):
     """One ViterbiRunner::alignment-style call with host buffers in and out.
@@ -876,16 +948,7 @@ def viterbi_search(ctx: Context, db: TargetDB, ids=None, exclusions=None, want_p
         paths = np.zeros(cap, np.uint8)
     if not want_paths:
         paths = None
-    eo = ei = ej = None
-    if exclusions is not None:
-        cnt = np.array([0 if e is None else len(e[0]) for e in exclusions], np.int64)
-        eo = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int64)
-        ei = np.concatenate([np.asarray(e[0], np.int32) for e in exclusions if e is not None] or
-                            [np.zeros(0, np.int32)]).astype(np.int32)
-        ej = np.concatenate([np.asarray(e[1], np.int32) for e in exclusions if e is not None] or
-                            [np.zeros(0, np.int32)]).astype(np.int32)
-        if len(ei) == 0:
-            ei = np.zeros(1, np.int32); ej = np.zeros(1, np.int32)
+    eo, ei, ej = _exclusions(exclusions)
     _ck(ctx.L.hhg_viterbi_search(ctx.h, db.h, n, _p(ids, c_i32p), hits.ctypes.data_as(C.c_void_p),
                                  _p(paths, c_u8p), cap if want_paths else 0, _p(eo, c_i64p), _p(ei, c_i32p),
                                  _p(ej, c_i32p)))
@@ -912,8 +975,10 @@ def query_set_batch(ctx: Context, queries, S33=None, q_pav=None, local=True, egq
     ctx.batch_Lq = Lq
 
 
-def viterbi_search_batch(ctx: Context, db: TargetDB, req_query, ids, columnscore=1, pb=None, want_paths=True):
-    """hhg_viterbi_search_batch: request k aligns query req_query[k] of the current batch with target ids[k]."""
+def viterbi_search_batch(ctx: Context, db: TargetDB, req_query, ids, columnscore=1, pb=None, want_paths=True,
+                         exclusions=None):
+    """hhg_viterbi_search_batch: request k aligns query req_query[k] of the current batch with target ids[k].
+    exclusions: optional list (per request) of (i_steps, j_steps) int arrays to mask, as in viterbi_search."""
     rq = np.ascontiguousarray(req_query, np.int32); ids = np.ascontiguousarray(ids, np.int32)
     n = len(ids)
     hits = np.zeros(n, HIT_DTYPE)
@@ -921,8 +986,10 @@ def viterbi_search_batch(ctx: Context, db: TargetDB, req_query, ids, columnscore
                      db.Lh[np.clip(ids, 0, db.n - 1)].astype(np.int64) + 2))
     paths = np.zeros(cap, np.uint8) if want_paths else None
     pbv = None if pb is None else np.ascontiguousarray(pb, np.float32)
+    eo, ei, ej = _exclusions(exclusions)
     _ck(ctx.L.hhg_viterbi_search_batch(ctx.h, db.h, n, _p(rq, c_i32p), _p(ids, c_i32p), columnscore, _p(pbv, c_f32p),
-                                       hits.ctypes.data_as(C.c_void_p), _p(paths, c_u8p), cap if want_paths else 0))
+                                       hits.ctypes.data_as(C.c_void_p), _p(paths, c_u8p), cap if want_paths else 0,
+                                       _p(eo, c_i64p), _p(ei, c_i32p), _p(ej, c_i32p)))
     return hits, paths
 
 

@@ -741,6 +741,32 @@ __global__ void k_null_model(long long total_cols, int n, const long long* col_o
   dst[6] = src[6];
 }
 
+// Template records of a MAC realignment over a raw shard (hhg_mac_realign_batch): request r's Lt[r] records are
+// copied from the raw records of target[r] into out + dst[r] (both in records), with the null model of its query
+// req_q[r] factored into the emissions by the same operations as k_null_model.  The realignment then reads its own
+// copy, whatever query hhg_db_apply_null_model last prepared the shard's `cols` for.  Grid: (x, requests).
+__global__ void k_mac_gather_cols(int n, const int* __restrict__ req_q, const int* __restrict__ target,
+                                  const int* __restrict__ Lt, const long long* __restrict__ col_off,
+                                  const long long* __restrict__ dst, const float4* __restrict__ raw,
+                                  const float* __restrict__ t_pav, const float* __restrict__ q_pav,
+                                  const float* __restrict__ pb, int columnscore, float4* __restrict__ out) {
+  const int r = blockIdx.y;
+  if (r >= n) return;
+  const int t = target[r], L = Lt[r];
+  float pn[20];
+  null_model_vec(columnscore, q_pav + (size_t)req_q[r] * 20, t_pav + (size_t)t * 20, pb, pn);
+  const float4* src0 = raw + (size_t)col_off[t] * 7;
+  float4* dst0 = out + (size_t)dst[r] * 7;
+  for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < L; c += gridDim.x * blockDim.x) {
+    const float4* src = src0 + (size_t)c * 7;
+    float4* d = dst0 + (size_t)c * 7;
+#pragma unroll
+    for (int k = 0; k < 5; ++k) d[k] = div4(src[k], pn + 4 * k);
+    d[5] = src[5];
+    d[6] = src[6];
+  }
+}
+
 // Compact the per-request path strings (capacity Lq+Lt+2 each) to their real lengths before the D2H copy:
 // one thread per request copies nsteps bytes to its compact offset.
 __global__ void k_gather_paths(int n, const HitRec* hits, const ReqDesc* reqs, const long long* dst_off,

@@ -12,7 +12,8 @@
 //   * within a row, MM / DG / MI depend on the previous row only  -> lanes = columns
 //   * GD and IM are first-order recurrences along the row          -> two lanes scan the row sequentially
 //   * the row maximum (scale factors) is order-independent         -> warp reduction
-//   * hits are independent                                         -> one warp each, all hits of a query concurrently
+//   * hits are independent                                         -> one warp each, all hits of a query (or of a
+//                                                                     batch of queries, MacArgs.req_q) concurrently
 // No secondary-structure term (hit.ssm2 == 0) and no self-alignment mode.
 #pragma once
 #include <cfloat>
@@ -58,11 +59,32 @@ struct MacArgs {
   const int* req_map;                  // optional: blockIdx.x -> request (launches over a subset of the requests)
   long long* dbg;                      // optional [n*12] per-phase clock64 totals (HHG_MAC_TIMING)
   int smem_rows;                       // bytes of dynamic shared memory available for the row buffers
-  double* scale;                       // [n*(Lq+3)]
+  double* scale;                       // [n*(Lq+3)], or per request at scale_off (query batch)
   MacHitOut* out;
   long long* path_off;                 // [n] into out_i/out_j/out_states/out_post
   int* out_i; int* out_j; uint8_t* out_states; float* out_post;
+  // query batch: request r realigns query req_q[r], of length q_L[q] with p at q_p + q_p_off[q] and transitions at
+  // q_tr + q_tr_off[q]; its scale factors sit at scale + scale_off[r].  req_q == nullptr (the zero value): every
+  // request uses the one query Lq / q_p / q_tr, scale factors at scale + r*(Lq+3).
+  const int* req_q;                    // [n] or nullptr
+  const int* q_L;                      // [nq]
+  const long long* q_p_off;            // [nq]
+  const long long* q_tr_off;           // [nq]
+  const long long* scale_off;          // [n]
 };
+
+struct MacQuery {
+  int Lq;
+  const float* p;                      // [(Lq+2)*20]
+  const float* tr;                     // [(Lq+1)*7]
+  double* scale;                       // [Lq+3]
+};
+
+__device__ __forceinline__ MacQuery mac_query(const MacArgs& A, int r) {
+  if (!A.req_q) return MacQuery{A.Lq, A.q_p, A.q_tr, A.scale + (size_t)r * (A.Lq + 3)};
+  const int q = A.req_q[r];
+  return MacQuery{A.q_L[q], A.q_p + A.q_p_off[q], A.q_tr + A.q_tr_off[q], A.scale + A.scale_off[r]};
+}
 
 __device__ __forceinline__ float mac_dot20(const float* __restrict__ qi, const float* __restrict__ tj) {
   float s = __fmul_rn(tj[0], qi[0]);                 // ScalarProd20, src/hhhit-inl.h:117-122: left to right
@@ -98,7 +120,7 @@ __global__ void k_mac_gather_tr(int n, const ColRec* __restrict__ cols, const lo
 // Cell-off band: block per request.
 __global__ void __launch_bounds__(256) k_mac_band(const MacArgs A) {
   const int r = blockIdx.x;
-  const int Lq = A.Lq, Lt = A.Lt[r], W = Lt + 1;
+  const int Lq = mac_query(A, r).Lq, Lt = A.Lt[r], W = Lt + 1;
   uint8_t* off = A.off + A.cell_off[r];
   const int i1 = A.vit[r * 5], i2 = A.vit[r * 5 + 1], j1 = A.vit[r * 5 + 2], j2 = A.vit[r * 5 + 3], ns = A.vit[r * 5 + 4];
   const long long total = (long long)(Lq + 1) * W;
@@ -156,14 +178,16 @@ __global__ void __launch_bounds__(256) k_mac_band(const MacArgs A) {
 __global__ void __launch_bounds__(32) k_mac_realign(const MacArgs A) {
   extern __shared__ __align__(16) unsigned char mac_smem[];
   const int r = A.req_map ? A.req_map[blockIdx.x] : (int)blockIdx.x, lane = threadIdx.x;
-  const int Lq = A.Lq, Lt = A.Lt[r], W = Lt + 1;
+  const MacQuery Q = mac_query(A, r);
+  const int Lq = Q.Lq, Lt = A.Lt[r], W = Lt + 1;
   const uint8_t* off = A.off + A.cell_off[r];
   uint8_t* bt = A.bt + A.cell_off[r];
   float* post = A.post + A.cell_off[r];
   const ColRec* tcol = A.cols + A.rec0[r] - 1;            // tcol[j] = record of column j (1-based)
   const float* ttr_g = A.t_tr + A.tr_off[r];
-  const float* qtr = A.q_tr;
-  double* scale = A.scale + (size_t)r * (Lq + 3);
+  const float* qtr = Q.tr;
+  const float* q_p = Q.p;
+  double* scale = Q.scale;
   const size_t RS = (size_t)Lt + 3;
   // per-warp working set: 10 row buffers (doubles), the template's linear transitions, the cell-off flags of the
   // current row.  In shared memory when it fits; the sequential scans below then never wait for global memory.
@@ -253,7 +277,7 @@ __global__ void __launch_bounds__(32) k_mac_realign(const MacArgs A) {
     for (int j = 1 + lane; j <= Lt; j += 32) {
       const uint8_t o = OFFC(1, j);
       offrow[j] = o;
-      if (!o) { Cm[j] = (double)mac_dot20(A.q_p + 20, tcol[j].p) * Cshift; lo = min(lo, j); hi = max(hi, j); }
+      if (!o) { Cm[j] = (double)mac_dot20(q_p + 20, tcol[j].p) * Cshift; lo = min(lo, j); hi = max(hi, j); }
     }
     row_span(lo, hi);
   }
@@ -272,7 +296,7 @@ __global__ void __launch_bounds__(32) k_mac_realign(const MacArgs A) {
   for (int i = 2; i <= Lq; ++i) {
     const double sc_i = scale[i];
     if (scale_prod < DBL_MIN * 100) scale_prod = 0.0; else scale_prod *= sc_i;
-    const float* qi = A.q_p + (size_t)i * 20;
+    const float* qi = q_p + (size_t)i * 20;
     const float q_m2m = QT(i - 1, M2M), q_i2m = QT(i - 1, I2M), q_d2m = QT(i - 1, D2M), q_m2d = QT(i - 1, M2D),
                 q_d2d = QT(i - 1, D2D);
     double pmax = 0.0;
@@ -349,7 +373,7 @@ __global__ void __launch_bounds__(32) k_mac_realign(const MacArgs A) {
     if (scale_prod < DBL_MIN * 100) scale_prod = 0.0;
     pmin *= sc_n;
     if (pmin < DBL_MIN * 100) pmin = 0.0;
-    const float* qn = A.q_p + (size_t)(i + 1) * 20;
+    const float* qn = q_p + (size_t)(i + 1) * 20;
     const float q_m2m = QT(i, M2M), q_m2i = QT(i, M2I), q_m2d = QT(i, M2D), q_i2m = QT(i, I2M), q_i2i = QT(i, I2I),
                 q_d2m = QT(i, D2M), q_d2d = QT(i, D2D);
     // phase A (lanes = columns): pmatch -> Cm (scratch), DG, MI; the cell in column Lt

@@ -118,3 +118,49 @@ class ViterbiRunner:
                 nxt.append(int(t))
                 # ExcludeAlignment masks steps 1 <= step < nsteps (src/hhviterbi.cpp:66)
                 excl.setdefault(int(t), []).append((gi[1:n].copy(), gj[1:n].copy()))
+
+
+class BatchViterbiRunner:
+    """ViterbiRunner.alignment for every query of a batch at once (hhblits_omp runs one ViterbiRunner per query,
+    src/hhblits_omp.cpp:119-160): pass 0 aligns every request, pass k > 0 realigns the (query, target) requests whose
+    previous hit scored above smin with all earlier paths of that pair masked -- one hhg_viterbi_search_batch call per
+    pass for all queries.  The queries are those of the last capi.query_set_batch; over a raw shard the null model is
+    applied per query (columnscore / pb as in capi.viterbi_search_batch).  No early stopping and no per-batch ss
+    consensus: split the requests by hhg_set_use_ss beforehand if the ss term is wanted for some of them."""
+
+    def __init__(self, ctx: capi.Context, db: capi.TargetDB, altali: int = 4, smin: float = 20.0, columnscore: int = 1,
+                 pb=None):
+        self.ctx, self.db = ctx, db
+        self.altali, self.smin = altali, smin
+        self.columnscore, self.pb = columnscore, pb
+
+    def alignment(self, req_query, ids) -> list[list[Hit]]:
+        """Request k aligns query req_query[k] with target ids[k].  Returns one list of Hits per query of the batch,
+        in the order ViterbiRunner.alignment(ids of that query) returns them."""
+        rq = np.ascontiguousarray(req_query, np.int32); ids = np.ascontiguousarray(ids, np.int32)
+        out: list[list[Hit]] = [[] for _ in range(len(self.ctx.batch_Lq))]
+        excl: dict[tuple[int, int], list[tuple[np.ndarray, np.ndarray]]] = {}
+        todo = list(zip(rq.tolist(), ids.tolist()))
+        for rep in range(self.altali):
+            if not todo:
+                break
+            exclusions = None
+            if rep > 0:
+                exclusions = [(np.concatenate([e[0] for e in excl[p]]), np.concatenate([e[1] for e in excl[p]]))
+                              for p in todo]
+            hits, paths = capi.viterbi_search_batch(self.ctx, self.db, [q for q, _ in todo], [t for _, t in todo],
+                                                    self.columnscore, self.pb, exclusions=exclusions)
+            nxt = []
+            for k, (q, t) in enumerate(todo):
+                h = hits[k]
+                gi, gj, gs = capi.expand_path(h, paths)
+                n = int(h["nsteps"])
+                out[q].append(Hit(t, rep + 1, 1 if h["hit_score"] <= self.smin else 0, float(h["hit_score"]),
+                                  float(h["score_ss"]), float(h["score"]), int(h["i1"]), int(h["i2"]), int(h["j1"]),
+                                  int(h["j2"]), n, int(h["matched_cols"]), gi, gj, gs))
+                if h["hit_score"] > self.smin:
+                    nxt.append((q, t))
+                    # ExcludeAlignment masks steps 1 <= step < nsteps (src/hhviterbi.cpp:66)
+                    excl.setdefault((q, t), []).append((gi[1:n].copy(), gj[1:n].copy()))
+            todo = nxt
+        return out

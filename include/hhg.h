@@ -18,6 +18,7 @@
  *   HHEntry::getTemplateHMM / HMM::Read src/hhdatabase.cpp:300, src/hhhmm.cpp:202 -> hhg_db_create_hhm
  *   PrepareTemplateHMM                  src/hhfunc.cpp:165         -> hhg_db_create_hhm + hhg_db_apply_null_model
  *   PosteriorDecoder::realign           src/hhposteriordecoder.h:67 -> hhg_mac_realign
+ *   PosteriorDecoderRunner (hhblits_omp, one per query)               -> hhg_mac_realign_batch
  *
  * Error convention: every function returns 0 on success or a negative HHG_E* code;
  * hhg_last_error() returns a thread-local message.  (The reference logs and exit()s,
@@ -295,8 +296,8 @@ int hhg_set_use_ss(hhg_ctx* ctx, int use_ss);
 /* -excl / -template_excl (par.exclstr, par.template_exclstr; ViterbiRunner::exclude_regions / exclude_template_regions,
  * src/hhviterbirunner.cpp:291-330): query rows q_lo[k]..q_hi[k] are switched off for every template column, template
  * columns t_lo[k]..t_hi[k] for every query row, in every following search of this context (1-based, inclusive; counts of
- * 0 clear the setting).  Works together with the excl_* path exclusions of hhg_viterbi_search, and applies to
- * hhg_mac_realign as well (PosteriorDecoder::exclude_regions / exclude_template_regions,
+ * 0 clear the setting).  Works together with the excl_* path exclusions of hhg_viterbi_search(_batch), and applies to
+ * hhg_mac_realign(_batch) as well (PosteriorDecoder::exclude_regions / exclude_template_regions,
  * src/hhposteriordecoder.cpp:100-152). */
 int hhg_set_excluded_regions(hhg_ctx* ctx, int nq, const int32_t* q_lo, const int32_t* q_hi, int nt, const int32_t* t_lo,
                              const int32_t* t_hi);
@@ -332,11 +333,15 @@ int hhg_viterbi_search(hhg_ctx* ctx, const hhg_db* db, int n, const int32_t* ids
  *                         hhg_viterbi_search (paths_cap >= sum(Lq_of_request + Lt + 2)).  Raw shard
  *                         (hhg_db_create_raw / _hhm / _packed): the query-dependent null model
  *                         (HMM::IncludeNullModelInHMM, columnscore / pb as in hhg_db_apply_null_model) is applied per
- *                         query while the plan's operand stream is built -- no per-query pass over the whole shard. */
+ *                         query while the plan's operand stream is built -- no per-query pass over the whole shard.
+ *                         excl_*: as in hhg_viterbi_search, per request (the alternative alignments of
+ *                         ViterbiRunner::alignment for every query of the batch in one call); steps are checked against
+ *                         that request's query length and target length.  NULL = no path exclusions. */
 int hhg_query_set_batch(hhg_ctx* ctx, int nq, const int32_t* Lq, const float* const* p, const float* const* tr,
                         const uint8_t* const* ss, const float* q_pav, const float* S33, const hhg_params* par);
 int hhg_viterbi_search_batch(hhg_ctx* ctx, const hhg_db* db, int n, const int32_t* req_query, const int32_t* ids,
-                             int columnscore, const float* pb, hhg_hit* hits, uint8_t* paths, size_t paths_cap);
+                             int columnscore, const float* pb, hhg_hit* hits, uint8_t* paths, size_t paths_cap,
+                             const int64_t* excl_off, const int32_t* excl_i, const int32_t* excl_j);
 
 /* Device-resident variant used for kernel-only timing: plan once, run many times, fetch at the end. */
 typedef struct hhg_plan hhg_plan;
@@ -438,7 +443,7 @@ int hhg_plan_debug_bt(hhg_ctx* ctx, hhg_plan* plan, int k, uint8_t* bt);
  * computed with the reference's operation order and types, so posteriors, Pforward and paths are bit-identical.
  * The secondary-structure term: for predicted-vs-predicted structure (hit.ssm2 = 3) the reference's ScoreSS switch has
  * no such case (HMM::PRED_PRED = 4) and contributes exactly 0, so those hits are exact; not covered: DSSP-annotated
- * templates (hit.ssm2 = 1 or 2), self-alignment (hit.self), exclstr regions.
+ * templates (hit.ssm2 = 1 or 2), self-alignment (hit.self).
  *
  * hhg_mac_query_set: q_p = HMM::p of the query, q_tr_lin = HMM::tr after Log2LinTransitionProbs(1.0)
  *   (src/hhposteriordecoderrunner.cpp:48); the boundary rows are reset here like initializeQueryHMMTransitions.
@@ -469,7 +474,28 @@ int hhg_mac_realign(hhg_ctx* ctx, const hhg_db* db, int n, const int32_t* target
                     const int64_t* vit_off, const int32_t* vit_i, const int32_t* vit_j, const int64_t* excl_off,
                     const int32_t* excl_i, const int32_t* excl_j, const hhg_mac_params* par, hhg_mac_hit* hits,
                     int32_t* out_i, int32_t* out_j, uint8_t* out_states, float* out_post, size_t path_cap);
-/* Debug / parity: the posterior matrix of request `request` of the last hhg_mac_realign, (Lq+1) x (Lt+1) floats. */
+
+/* Query batches (hhblits_omp runs one PosteriorDecoderRunner::executeComputation per query,
+ * src/hhblits.cpp:973-1063 perform_realign): the hits of many queries realigned in one call.
+ * hhg_mac_query_set_batch: nq queries as in hhg_mac_query_set; q_pav[nq*20] = HMM::pav of each query, needed when the
+ *   shard is raw (may be NULL otherwise).  hhg_mac_query_set == a batch of one without q_pav.
+ * hhg_mac_realign_batch, request r: query req_query[r] against target[r]; every other argument as in hhg_mac_realign,
+ *   path_cap >= sum(Lq of the request's query + Lt + 2).  Raw shard (hhg_db_create_raw / _hhm / _packed): the null
+ *   model of the request's query (HMM::IncludeNullModelInHMM, columnscore / pb as in hhg_viterbi_search_batch) is
+ *   applied to a copy of the template's raw records, so the result does not depend on hhg_db_apply_null_model; a
+ *   prepared shard is read as it is and columnscore / pb are ignored.  The requests are cut, in order, into memory waves
+ *   whose scratch (about 6 bytes per cell) stays within the context's backtrace budget (HHG_MAX_BT_GB); the results
+ *   do not depend on the cut.  Results are bit-identical to hhg_db_apply_null_model + hhg_mac_query_set +
+ *   hhg_mac_realign per query. */
+int hhg_mac_query_set_batch(hhg_ctx* ctx, int nq, const int32_t* Lq, const float* const* q_p,
+                            const float* const* q_tr_lin, const float* q_pav);
+int hhg_mac_realign_batch(hhg_ctx* ctx, const hhg_db* db, int n, const int32_t* req_query, const int32_t* target,
+                          const int32_t* vit, const int64_t* vit_off, const int32_t* vit_i, const int32_t* vit_j,
+                          const int64_t* excl_off, const int32_t* excl_i, const int32_t* excl_j,
+                          int columnscore, const float* pb, const hhg_mac_params* par, hhg_mac_hit* hits,
+                          int32_t* out_i, int32_t* out_j, uint8_t* out_states, float* out_post, size_t path_cap);
+/* Debug / parity: the posterior matrix of request `request` of the last hhg_mac_realign(_batch), (Lq+1) x (Lt+1)
+ * floats with the request's own Lq.  Refused after a call that ran in more than one memory wave. */
 int hhg_mac_debug_posterior(hhg_ctx* ctx, int request, float* out);
 
 /* ---- cs219 ungapped prefilter (stage 1 of Prefilter::prefilter_db, src/hhprefilter.cpp:466-482) */
