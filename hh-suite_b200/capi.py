@@ -48,7 +48,9 @@ SYMBOLS = ["hhg_last_error", "hhg_ctx_create", "hhg_ctx_destroy", "hhg_ctx_sync"
            "hhg_msa_params_default", "hhg_a3m_scan", "hhg_a3m_parse", "hhg_msa_to_hmm", "hhg_db_create_a3m", "hhg_query_from_a3m",
            "hhg_ca3m_scan", "hhg_ca3m_parse", "hhg_ca3m_to_hmm", "hhg_db_create_ca3m",
            "hhg_crf_create", "hhg_crf_destroy", "hhg_crf_info", "hhg_query_context_pseudocounts", "hhg_crf_parse_host",
-           "hhg_crf_state", "hhg_crf_tail_host", "hhg_context_library_create", "hhg_context_library_parse_host"]
+           "hhg_crf_state", "hhg_crf_tail_host", "hhg_context_library_create", "hhg_context_library_parse_host",
+           "hhg_prefilter_ungapped_batch_run", "hhg_prefilter_ungapped_batch_fetch", "hhg_prefilter_select_batch",
+           "hhg_prefilter_sw_batch", "hhg_prefilter_batch_max_queries"]
 
 
 class PrepParams(C.Structure):
@@ -283,6 +285,14 @@ def load():
                                         C.POINTER(C.c_double)]
     L.hhg_prefilter_sw.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, C.c_int, c_u8p, C.c_int, C.c_int, C.c_int,
                                    c_i32p]
+    L.hhg_prefilter_ungapped_batch_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, C.POINTER(C.c_void_p),
+                                                   C.c_int]
+    L.hhg_prefilter_ungapped_batch_fetch.argtypes = [C.c_void_p, C.c_void_p, c_i32p]
+    L.hhg_prefilter_batch_max_queries.argtypes = [C.c_void_p, C.c_void_p]
+    L.hhg_prefilter_select_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, c_i32p,
+                                             c_i32p, C.c_int, c_i32p]
+    L.hhg_prefilter_sw_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, C.POINTER(C.c_void_p), C.c_int, c_i32p,
+                                         c_i32p, C.c_int, C.c_int, C.c_int, c_i32p]
     L.hhg_comm_unique_id.argtypes = [C.c_void_p]
     L.hhg_comm_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
     L.hhg_comm_destroy.argtypes = [C.c_void_p]
@@ -1024,6 +1034,15 @@ def build_prefilter_profile(q_p, q_pav, lib219, offset=50, bit_factor=4):
     return prof
 
 
+def _profile_batch(profs):
+    """(contiguous uint8 profiles, their lengths, the array of their addresses) as the batch prefilter calls take them;
+    the profiles must stay referenced for the duration of the call."""
+    profs = [np.ascontiguousarray(p, np.uint8) for p in profs]
+    assert all(p.ndim == 2 and p.shape[0] == 220 for p in profs)
+    Lq = np.array([p.shape[1] for p in profs], np.int32)
+    return profs, Lq, (C.c_void_p * max(len(profs), 1))(*[p.ctypes.data for p in profs])
+
+
 class CsDB:
     def __init__(self, ctx: Context, L, off, seq):
         self.ctx = ctx
@@ -1083,6 +1102,48 @@ class CsDB:
     def fetch(self):
         sc = np.zeros(self.n, np.int32)
         _ck(self.ctx.L.hhg_prefilter_fetch(self.ctx.h, self.h, _p(sc, c_i32p)))
+        return sc
+
+    # ---- query batches: each call equals the single-query call above made once per profile
+    def max_batch(self) -> int:
+        """Queries whose score rows fit the context's memory budget in one run_batch (at least 1)."""
+        return int(self.ctx.L.hhg_prefilter_batch_max_queries(self.ctx.h, self.h))
+
+    def run_batch(self, profs, offset=50):
+        """hhg_prefilter_ungapped_batch_run: raw ungapped scores of every profile, left on the device."""
+        profs, Lq, ptrs = _profile_batch(profs)
+        _ck(self.ctx.L.hhg_prefilter_ungapped_batch_run(self.ctx.h, self.h, len(profs), _p(Lq, c_i32p), ptrs, offset))
+
+    def fetch_batch(self, nq):
+        """Raw scores of the last run_batch (nq profiles): [nq, n]."""
+        sc = np.zeros((nq, self.n), np.int32)
+        _ck(self.ctx.L.hhg_prefilter_ungapped_batch_fetch(self.ctx.h, self.h, _p(sc, c_i32p)))
+        return sc
+
+    def ungapped_batch(self, profs, offset=50):
+        self.run_batch(profs, offset)
+        return self.fetch_batch(len(profs))
+
+    def select_batch(self, Lq, bit_factor=4, smax_thresh=10, min_hits=100, cap=None):
+        """Stage-1 selection of every query of the last run_batch: one (ids, corrected scores) pair per query, each
+        equal to select().  cap: total output capacity (default: every sequence for every query)."""
+        Lq = np.ascontiguousarray(Lq, np.int32)
+        nq = len(Lq)
+        cap = nq * self.n if cap is None else int(cap)
+        ids = np.empty(max(cap, 1), np.int32); sc = np.empty(max(cap, 1), np.int32); off = np.zeros(nq + 1, np.int32)
+        _ck(self.ctx.L.hhg_prefilter_select_batch(self.ctx.h, self.h, nq, _p(Lq, c_i32p), bit_factor, smax_thresh,
+                                                  min_hits, _p(ids, c_i32p), _p(sc, c_i32p), cap, _p(off, c_i32p)))
+        return [(ids[off[q]:off[q + 1]].copy(), sc[off[q]:off[q + 1]].copy()) for q in range(nq)]
+
+    def sw_batch(self, profs, req_query, ids, gap_open=24, gap_extend=4, bias=50):
+        """Stage-2 gapped scores of request k = profile req_query[k] against sequence ids[k], in one launch."""
+        profs, Lq, ptrs = _profile_batch(profs)
+        rq = np.ascontiguousarray(req_query, np.int32); ids = np.ascontiguousarray(ids, np.int32)
+        assert len(rq) == len(ids)
+        sc = np.zeros(len(ids), np.int32)
+        _ck(self.ctx.L.hhg_prefilter_sw_batch(self.ctx.h, self.h, len(profs), _p(Lq, c_i32p), ptrs, len(ids),
+                                              _p(rq, c_i32p), _p(ids, c_i32p), gap_open, gap_extend, bias,
+                                              _p(sc, c_i32p)))
         return sc
 
     def close(self):

@@ -20,7 +20,36 @@ def search(ctx: capi.Context, db: capi.TargetDB, csdb: capi.CsDB, q_p, q_tr, q_p
     checked as far as it can be (same number of entries, same lengths)."""
     prof = capi.build_prefilter_profile(q_p if q_prefilter_p is None else q_prefilter_p, q_pav, lib219,
                                         pf_kwargs.get("score_offset", 50), pf_kwargs.get("bit_factor", 4))
-    ids = prefilter.prefilter_db(csdb, prof, **pf_kwargs)
+    ids = _to_targets(prefilter.prefilter_db(csdb, prof, **pf_kwargs), db, csdb, cs_names, db_names)
+    ctx.set_query(q_p, q_tr)
+    hits = runner.ViterbiRunner(ctx, db, altali=altali, smin=smin).alignment(ids) if len(ids) else []
+    return ids, hits
+
+
+def search_batch(ctx: capi.Context, db: capi.TargetDB, csdb: capi.CsDB, queries, lib219, altali=4, smin=20.0,
+                 cs_names=None, db_names=None, **pf_kwargs):
+    """search() for many queries against one database (hhblits_omp): queries = list of (q_p, q_tr, q_pav) or
+    (q_p, q_tr, q_pav, q_prefilter_p).  The prefilter of all queries runs as one batch
+    (prefilter.prefilter_db_batch), the survivors are mapped to the target shard as in search(), and the Viterbi
+    stage aligns every query with its own survivors through capi.query_set_batch and runner.BatchViterbiRunner.
+    Returns one (survivor ids in the TARGET shard, list of runner.Hit) pair per query.
+
+    BatchViterbiRunner has no early stopping and no per-8-lane ss consensus, unlike runner.ViterbiRunner; search()
+    uses neither, so the results equal [search(ctx, db, csdb, *q, lib219, ...) for q in queries] for the settings the
+    two runners share.  The batch replaces the context's query (capi.query_set_batch)."""
+    so, bf = pf_kwargs.get("score_offset", 50), pf_kwargs.get("bit_factor", 4)
+    profs = [capi.build_prefilter_profile(q[0] if len(q) < 4 or q[3] is None else q[3], q[2], lib219, so, bf)
+             for q in queries]
+    ids = [_to_targets(x, db, csdb, cs_names, db_names) for x in prefilter.prefilter_db_batch(csdb, profs, **pf_kwargs)]
+    capi.query_set_batch(ctx, [(q[0], q[1]) for q in queries])
+    rq = np.concatenate([np.full(len(x), q, np.int32) for q, x in enumerate(ids)])
+    hits = runner.BatchViterbiRunner(ctx, db, altali=altali, smin=smin).alignment(rq, np.concatenate(ids)) \
+        if len(rq) else [[] for _ in queries]
+    return list(zip(ids, hits))
+
+
+def _to_targets(ids, db, csdb, cs_names, db_names):
+    """Prefilter survivors (cs219 index) -> target shard index, by name when the name lists are given."""
     if cs_names is not None or db_names is not None:
         if cs_names is None or db_names is None:
             raise ValueError("pass both cs_names and db_names, or neither")
@@ -28,13 +57,11 @@ def search(ctx: capi.Context, db: capi.TargetDB, csdb: capi.CsDB, q_p, q_tr, q_p
         missing = [cs_names[k] for k in ids if cs_names[k] not in where]
         if missing:
             raise KeyError(f"{len(missing)} prefilter hits have no entry in the profile shard, e.g. {missing[0]!r}")
-        ids = np.array([where[cs_names[k]] for k in ids], np.int32)
-    elif csdb.n != db.n or not np.array_equal(np.asarray(csdb.Lh), np.asarray(db.Lh)):
+        return np.array([where[cs_names[k]] for k in ids], np.int32)
+    if csdb.n != db.n or not np.array_equal(np.asarray(csdb.Lh), np.asarray(db.Lh)):
         raise ValueError("cs219 shard and profile shard are not index-aligned (different sizes or lengths): "
                          "pass cs_names / db_names so the survivors are mapped by name like the reference does")
-    ctx.set_query(q_p, q_tr)
-    hits = runner.ViterbiRunner(ctx, db, altali=altali, smin=smin).alignment(ids) if len(ids) else []
-    return ids, hits
+    return ids
 
 
 def translate_cs219(p_cols: np.ndarray, pav_like: np.ndarray, lib219: np.ndarray) -> np.ndarray:

@@ -51,11 +51,21 @@ def prefilter_db(csdb: capi.CsDB, prof: np.ndarray, gap_open=20, gap_extend=4, s
         first_scores = corr32[first]
     sw = csdb.sw(prof, ids=first, gap_open=gap_open + gap_extend, gap_extend=gap_extend, bias=score_offset) \
         if len(first) else np.zeros(0, np.int32)
+    ids, ev = _stage2(csdb, Lq, first, sw, bit_factor, evalue_thresh, evalue_coarse_thresh, min_prefilter_hits, maxnumdb)
+    if return_details:
+        return ids, dict(raw=raw, corrected=corr, first=first, first_scores=first_scores, sw=sw, evalue=ev)
+    return ids
+
+
+def _stage2(csdb, Lq, first, sw, bit_factor, evalue_thresh, evalue_coarse_thresh, min_prefilter_hits, maxnumdb):
+    """E-values of the stage-2 scores and the final cut (:529-590) on the host: (ids, evalues)."""
+    import ctypes as C
+    L = capi.load()
     ev = np.zeros(len(first), np.float64)
     if len(first):
         sw32 = np.ascontiguousarray(sw, np.int32)
-        fl = np.ascontiguousarray(lens32[first])
-        capi._ck(L.hhg_prefilter_evalues(len(first), capi._p(sw32, capi.c_i32p), capi._p(fl, capi.c_i32p), n, Lq,
+        fl = np.ascontiguousarray(np.asarray(csdb.Lh, np.int32)[first])
+        capi._ck(L.hhg_prefilter_evalues(len(first), capi._p(sw32, capi.c_i32p), capi._p(fl, capi.c_i32p), csdb.n, Lq,
                                         bit_factor, ev.ctypes.data_as(C.POINTER(C.c_double))))
     # coarse cut (:530), sort ascending by ((int)evalue, index) (:545), keep rule (:547-558), maxnumdb (:590) -- vectorised
     keep = np.nonzero(ev < evalue_coarse_thresh)[0]
@@ -63,7 +73,29 @@ def prefilter_db(csdb: capi.CsDB, prof: np.ndarray, gap_open=20, gap_extend=4, s
     tail = np.nonzero(ev[order[min_prefilter_hits:]] > evalue_thresh)[0]
     ncut = min_prefilter_hits + int(tail[0]) if len(tail) else len(order)
     out = order[:min(ncut, maxnumdb)]
-    ids = first[out] if len(out) else np.zeros(0, np.int32)
-    if return_details:
-        return ids, dict(raw=raw, corrected=corr, first=first, first_scores=first_scores, sw=sw, evalue=ev)
-    return ids
+    return (first[out] if len(out) else np.zeros(0, np.int32)), ev
+
+
+def prefilter_db_batch(csdb: capi.CsDB, profs, gap_open=20, gap_extend=4, score_offset=50, bit_factor=4,
+                       evalue_thresh=1000.0, evalue_coarse_thresh=100000.0, smax_thresh=10, min_prefilter_hits=100,
+                       maxnumdb=20000) -> list[np.ndarray]:
+    """prefilter_db for many queries against one shard (hhblits_omp): one ungapped batch run, one stage-1 selection
+    and one stage-2 launch for all queries, then each query's E-values and final cut on the host.  Returns one id
+    array per profile, equal to [prefilter_db(csdb, p, ...) for p in profs].  A batch whose score rows exceed the
+    context's memory budget (HHG_MAX_BT_GB) runs in consecutive groups of csdb.max_batch() queries."""
+    profs = [np.ascontiguousarray(p, np.uint8) for p in profs]
+    kw = dict(gap_open=gap_open, gap_extend=gap_extend, score_offset=score_offset, bit_factor=bit_factor,
+              evalue_thresh=evalue_thresh, evalue_coarse_thresh=evalue_coarse_thresh, smax_thresh=smax_thresh,
+              min_prefilter_hits=min_prefilter_hits, maxnumdb=maxnumdb)
+    group = csdb.max_batch()
+    if len(profs) > group:
+        return [ids for g in range(0, len(profs), group) for ids in prefilter_db_batch(csdb, profs[g:g + group], **kw)]
+    Lq = [p.shape[1] for p in profs]
+    csdb.run_batch(profs, score_offset)
+    firsts = [f for f, _ in csdb.select_batch(Lq, bit_factor, smax_thresh, min_prefilter_hits)]
+    rq = np.concatenate([np.full(len(f), q, np.int32) for q, f in enumerate(firsts)])
+    sw = csdb.sw_batch(profs, rq, np.concatenate(firsts), gap_open=gap_open + gap_extend, gap_extend=gap_extend,
+                       bias=score_offset)
+    bounds = np.concatenate([[0], np.cumsum([len(f) for f in firsts])])
+    return [_stage2(csdb, Lq[q], firsts[q], sw[bounds[q]:bounds[q + 1]], bit_factor, evalue_thresh,
+                    evalue_coarse_thresh, min_prefilter_hits, maxnumdb)[0] for q in range(len(profs))]

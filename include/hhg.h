@@ -548,6 +548,36 @@ int hhg_prefilter_evalues(int n, const int32_t* score, const int32_t* L, long lo
 int hhg_prefilter_sw(hhg_ctx* ctx, const hhg_csdb* db, int n, const int32_t* ids, int Lq,
                      const uint8_t* prof, int gap_open, int gap_extend, int bias, int32_t* scores);
 
+/* ---- cs219 prefilter for a batch of queries (hhblits_omp: one Prefilter::prefilter_db per query,
+ * src/hhblits_omp.cpp).  Each call equals the single-query call made once per query, element by element.
+ * prof[q]: uint8[220*Lq[q]] linear profile of query q, as hhg_prefilter_build_profile writes it.  All input is checked
+ * before anything launches; bad input (nq < 1, a length < 1, a NULL profile, an offset outside 0..255, a request's
+ * query or id out of range) returns HHG_EINVAL.
+ *
+ * hhg_prefilter_ungapped_batch_run: the ungapped stage of hhg_prefilter_ungapped for nq queries (nq <= 65535).  The
+ * nq x n raw scores stay on the device in context scratch (hhg_csdb's single-query scores are not touched) until the
+ * next batch run; hhg_prefilter_ungapped_batch_fetch copies them out, scores[q*n + k] = sequence k against query q.
+ * Queries of up to 512 positions share one pass over the shard; a longer query takes one launch per 512 positions.
+ * The nq x n score rows (raw and corrected, 8 bytes per query and sequence) must fit the context's memory budget
+ * (HHG_MAX_BT_GB): a larger batch is refused with HHG_EINVAL, and hhg_prefilter_batch_max_queries says how many queries
+ * fit (at least 1).  The edge bytes of long queries are cut into memory waves within what the score rows leave. */
+int hhg_prefilter_batch_max_queries(hhg_ctx* ctx, const hhg_csdb* db);
+int hhg_prefilter_ungapped_batch_run(hhg_ctx* ctx, const hhg_csdb* db, int nq, const int32_t* Lq,
+                                     const uint8_t* const* prof, int offset);
+int hhg_prefilter_ungapped_batch_fetch(hhg_ctx* ctx, const hhg_csdb* db, int32_t* scores);
+/* hhg_prefilter_select_batch: hhg_prefilter_select for every query of the last batch run on this shard (nq must match
+ * it), in two launches and two copies to the host whatever nq is.  Query q's survivors go to ids/scores[off[q] ..
+ * off[q+1]) in the reference's order; off[nq+1] is filled even when the call fails because off[nq] exceeds cap
+ * (HHG_EINVAL), so off[nq] is the capacity needed. */
+int hhg_prefilter_select_batch(hhg_ctx* ctx, const hhg_csdb* db, int nq, const int32_t* Lq, int bit_factor,
+                               int smax_thresh, int min_hits, int32_t* ids, int32_t* scores, int cap, int32_t* off);
+/* hhg_prefilter_sw_batch: hhg_prefilter_sw for n requests in one launch; request r scores query req_query[r] against
+ * sequence ids[r], scores[r] its result.  n = 0 is a no-op.  Same query length limit as hhg_prefilter_sw, checked for
+ * the whole batch. */
+int hhg_prefilter_sw_batch(hhg_ctx* ctx, const hhg_csdb* db, int nq, const int32_t* Lq, const uint8_t* const* prof,
+                           int n, const int32_t* req_query, const int32_t* ids, int gap_open, int gap_extend, int bias,
+                           int32_t* scores);
+
 #ifdef __cplusplus
 }
 #endif
