@@ -50,7 +50,10 @@ SYMBOLS = ["hhg_last_error", "hhg_ctx_create", "hhg_ctx_destroy", "hhg_ctx_sync"
            "hhg_crf_create", "hhg_crf_destroy", "hhg_crf_info", "hhg_query_context_pseudocounts", "hhg_crf_parse_host",
            "hhg_crf_state", "hhg_crf_tail_host", "hhg_context_library_create", "hhg_context_library_parse_host",
            "hhg_prefilter_ungapped_batch_run", "hhg_prefilter_ungapped_batch_fetch", "hhg_prefilter_select_batch",
-           "hhg_prefilter_sw_batch", "hhg_prefilter_batch_max_queries"]
+           "hhg_prefilter_sw_batch", "hhg_prefilter_batch_max_queries",
+           "hhg_dbstore_create", "hhg_dbstore_append_packed", "hhg_dbstore_append_db", "hhg_dbstore_destroy",
+           "hhg_dbstore_size", "hhg_dbstore_columns", "hhg_dbstore_lengths", "hhg_db_create_staged", "hhg_db_stage",
+           "hhg_db_staged_lookup"]
 
 
 class PrepParams(C.Structure):
@@ -351,6 +354,17 @@ def load():
     L.hhg_plan_topk_paths.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, c_u8p]
     L.hhg_ctx_last_plan.argtypes = [C.c_void_p]
     L.hhg_ctx_last_plan.restype = C.c_void_p
+    L.hhg_dbstore_create.argtypes = [C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.POINTER(C.c_void_p)]
+    L.hhg_dbstore_append_packed.argtypes = [C.c_void_p, C.c_int, c_i32p, C.c_void_p, c_f32p]
+    L.hhg_dbstore_append_db.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.hhg_dbstore_destroy.argtypes = [C.c_void_p]
+    L.hhg_dbstore_size.argtypes = [C.c_void_p]
+    L.hhg_dbstore_columns.argtypes = [C.c_void_p]
+    L.hhg_dbstore_columns.restype = C.c_longlong
+    L.hhg_dbstore_lengths.argtypes = [C.c_void_p, c_i32p]
+    L.hhg_db_create_staged.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.POINTER(C.c_void_p)]
+    L.hhg_db_stage.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, c_i32p, C.c_void_p]
+    L.hhg_db_staged_lookup.argtypes = [C.c_void_p, C.c_int, c_i32p, c_i32p, c_i64p]
     _lib = L
     return L
 
@@ -784,6 +798,97 @@ class TargetDB:
         if self.h:
             self.ctx.L.hhg_db_destroy(self.h)
             self.h = None
+
+
+class HostStore:
+    """The raw records of a whole database in page-locked, device-mapped host memory (hhg_dbstore): what a StagedDB
+    stages from.  Targets are numbered in append order (global ids)."""
+
+    def __init__(self, ctx: Context, capacity_targets: int, capacity_cols: int, has_ss: bool = False):
+        self.ctx = ctx
+        h = C.c_void_p()
+        _ck(ctx.L.hhg_dbstore_create(ctx.h, capacity_targets, capacity_cols, 1 if has_ss else 0, C.byref(h)))
+        self.h = h
+
+    @property
+    def n(self) -> int:
+        return int(self.ctx.L.hhg_dbstore_size(self.h))
+
+    @property
+    def columns(self) -> int:
+        return int(self.ctx.L.hhg_dbstore_columns(self.h))
+
+    @property
+    def Lh(self):
+        out = np.zeros(self.n, np.int32)
+        _ck(self.ctx.L.hhg_dbstore_lengths(self.h, _p(out, c_i32p)))
+        return out
+
+    def append_packed(self, L, cols_raw, pav):
+        """Host arrays in the format TargetDB.read_cols(0) / read_pav() return."""
+        L = np.ascontiguousarray(L, np.int32)
+        cols_raw = np.ascontiguousarray(cols_raw)
+        assert cols_raw.dtype == COLREC_DTYPE and len(cols_raw) == int(L.sum())
+        pav = np.ascontiguousarray(pav, np.float32)
+        assert pav.shape == (len(L), 20)
+        _ck(self.ctx.L.hhg_dbstore_append_packed(self.h, len(L), _p(L, c_i32p), cols_raw.ctypes.data_as(C.c_void_p),
+                                                 _p(pav, c_f32p)))
+
+    def append_db(self, db: "TargetDB"):
+        """All targets of a raw device shard (any loader): load a chunk, append it, close it."""
+        _ck(self.ctx.L.hhg_dbstore_append_db(self.ctx.h, self.h, db.h))
+
+    @classmethod
+    def from_db(cls, ctx: Context, db: "TargetDB", has_ss: bool = False):
+        self = cls(ctx, db.n, int(ctx.L.hhg_db_columns(db.h)), has_ss)
+        self.append_db(db)
+        return self
+
+    def close(self):
+        if self.h:
+            _ck(self.ctx.L.hhg_dbstore_destroy(self.h))
+            self.h = None
+
+
+STAGE_STATS_DTYPE = np.dtype([("hits", np.int64), ("copied", np.int64), ("bytes", np.int64), ("evicted", np.int64)])
+
+
+class StagedDB(TargetDB):
+    """A TargetDB of max_targets slots that caches targets of a HostStore (hhg_db_create_staged).  Every TargetDB use
+    works on it with LOCAL ids (slots); stage() makes targets resident, to_global() translates back.  n is the number
+    of slots, Lh the length of the target in each slot (0: empty)."""
+
+    def __init__(self, ctx: Context, store: HostStore, max_targets: int, max_cols: int):
+        h = C.c_void_p()
+        _ck(ctx.L.hhg_db_create_staged(ctx.h, store.h, max_targets, max_cols, C.byref(h)))
+        self.ctx, self.h, self.n, self.store = ctx, h, max_targets, store
+        self.Lh = np.zeros(max_targets, np.int32)
+        self.last_stats = np.zeros(1, STAGE_STATS_DTYPE)[0]
+
+    def stage(self, ids) -> np.ndarray:
+        """Make the store's targets ids resident (hhg_db_stage); returns their local ids.  last_stats: what it cost."""
+        ids = np.ascontiguousarray(ids, np.int32)
+        local = np.zeros(len(ids), np.int32)
+        stats = np.zeros(1, STAGE_STATS_DTYPE)
+        _ck(self.ctx.L.hhg_db_stage(self.ctx.h, self.h, len(ids), _p(ids, c_i32p), _p(local, c_i32p),
+                                    stats.ctypes.data_as(C.c_void_p)))
+        self.last_stats = stats[0]
+        _ck(self.ctx.L.hhg_db_lengths(self.h, _p(self.Lh, c_i32p)))
+        return local
+
+    def lookup(self, local):
+        """(global ids, first arena column) of local ids; global id -1 = empty slot."""
+        local = np.ascontiguousarray(local, np.int32)
+        g = np.zeros(len(local), np.int32); first = np.zeros(len(local), np.int64)
+        _ck(self.ctx.L.hhg_db_staged_lookup(self.h, len(local), _p(local, c_i32p), _p(g, c_i32p), _p(first, c_i64p)))
+        return g, first
+
+    def to_global(self, local) -> np.ndarray:
+        return self.lookup(local)[0]
+
+    def read_target(self, local: int):
+        """Raw column records of the target in slot `local`."""
+        return self.read_cols(0, int(self.lookup([local])[1][0]), int(self.Lh[local]))
 
 
 class Comm:

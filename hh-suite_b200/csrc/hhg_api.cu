@@ -9,6 +9,7 @@
 #include "hhg_mac.cuh"
 #include "hhg_topk.cuh"
 #include "hhg_hitlist.h"
+#include "hhg_stage_cache.h"
 
 #include <dlfcn.h>
 #if defined(__SSE__)
@@ -191,8 +192,24 @@ struct hhg_ctx {
 
 static std::atomic<unsigned long long> g_db_serial{1};
 
+// Page-locked, device-mapped host memory holding the raw records of a whole database (hhg_dbstore_*).
+struct hhg_dbstore {
+  int device = 0;
+  bool has_ss = false;
+  int cap_targets = 0, n = 0;
+  long long cap_cols = 0, total_cols = 0;
+  std::vector<int> L;
+  std::vector<long long> col_off;
+  ColRec* cols = nullptr;        // host addresses (cudaHostAlloc, mapped) ...
+  float* pav = nullptr;
+  const float4* d_cols = nullptr;   // ... and what the device calls them
+  const float* d_pav = nullptr;
+  int users = 0;                 // staged shards made over this store
+};
+
 struct hhg_db {
-  const unsigned long long serial = g_db_serial.fetch_add(1);   // identity for plan reuse (addresses get recycled)
+  // identity for plan reuse (addresses get recycled); a staged shard takes a new one whenever hhg_db_stage changes a slot
+  unsigned long long serial = g_db_serial.fetch_add(1);
   int device = 0;
   int n = 0;
   long long total_cols = 0;
@@ -207,6 +224,11 @@ struct hhg_db {
   DevBuf<float> pav;         // [n*20] template average aa frequencies
   bool prepared = true;
   unsigned long long cols_version = 1;   // bumped whenever `cols` is rewritten (hhg_db_apply_null_model)
+  // staged shard (hhg_db_create_staged): n slots over an arena of total_cols records; L[s] == 0 marks an empty slot
+  hhg_dbstore* store = nullptr;
+  std::unique_ptr<StageCache> stage;
+  DevBuf<StageDesc> d_desc;
+  DevBuf<int> d_slot_id, d_zero;         // 0..n-1 and zeros: k_mac_gather_cols' request arrays for a pass over all slots
 };
 
 struct hhg_csdb {
@@ -359,6 +381,15 @@ int hhg_ctx_sync(hhg_ctx* ctx) {
 
 long long hhg_ctx_launch_count(hhg_ctx* ctx) { return ctx ? ctx->launches : 0; }
 
+// The context's second stream and its two events, made on first use (long-template MAC launch, hhg_db_stage).
+static int ctx_aux_stream(hhg_ctx* ctx) {
+  if (ctx->aux_stream) return HHG_OK;
+  CK(cudaStreamCreateWithFlags(&ctx->aux_stream, cudaStreamNonBlocking));
+  CK(cudaEventCreateWithFlags(&ctx->aux_ev[0], cudaEventDisableTiming));
+  CK(cudaEventCreateWithFlags(&ctx->aux_ev[1], cudaEventDisableTiming));
+  return HHG_OK;
+}
+
 // ------------------------------------------------------------------------------------------ DB
 static int pack_profiles(hhg_ctx* ctx, int n, const int32_t* L, const int64_t* p_off,
                          const int64_t* tr_off, const int64_t* ss_off, const float* p, const float* tr,
@@ -510,11 +541,23 @@ int hhg_db_apply_null_model(hhg_ctx* ctx, hhg_db* db, const float* q_pav, const 
   if (q_pav) memcpy(h, q_pav, 80);
   if (pb) memcpy(h + 20, pb, 80);
   CK(cudaMemcpyAsync(dq.p, h, 160, cudaMemcpyHostToDevice, ctx->stream));
-  const int threads = 128;
-  k_null_model<<<(unsigned)((db->total_cols + threads - 1) / threads), threads, 0, ctx->stream>>>(
-      db->total_cols, db->n, db->dcol_off.p, db->cols_raw.p, db->pav.p, dq.p, dq.p + 20, columnscore,
-      db->cols.p);
-  ctx->launches++;
+  if (db->stage) {
+    // arena runs are in no order, so k_null_model's bisection over col_off does not apply: one k_mac_gather_cols
+    // "request" per slot with query 0 copies the slot's records in place of the arena (empty slots have L = 0)
+    for (int s0 = 0; s0 < db->n; s0 += 65535) {
+      const int k = std::min(db->n - s0, 65535);
+      k_mac_gather_cols<<<dim3(4, k), 128, 0, ctx->stream>>>(k, db->d_zero.p, db->d_slot_id.p + s0, db->dL.p + s0,
+                                                             db->dcol_off.p, db->dcol_off.p + s0, db->cols_raw.p, db->pav.p,
+                                                             dq.p, dq.p + 20, columnscore, db->cols.p);
+      ctx->launches++;
+    }
+  } else {
+    const int threads = 128;
+    k_null_model<<<(unsigned)((db->total_cols + threads - 1) / threads), threads, 0, ctx->stream>>>(
+        db->total_cols, db->n, db->dcol_off.p, db->cols_raw.p, db->pav.p, dq.p, dq.p + 20, columnscore,
+        db->cols.p);
+    ctx->launches++;
+  }
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(ctx->stream));
   db->prepared = true;
@@ -1399,7 +1442,11 @@ int hhg_debug_fastlog2_table(hhg_ctx* ctx, float* lg2_out) {
 }
 
 int hhg_db_destroy(hhg_db* db) {
-  if (db) { cudaSetDevice(db->device); delete db; }
+  if (db) {
+    cudaSetDevice(db->device);
+    if (db->store) db->store->users--;
+    delete db;
+  }
   return HHG_OK;
 }
 int hhg_db_size(const hhg_db* db) { return db ? db->n : 0; }
@@ -1408,6 +1455,220 @@ long long hhg_db_columns(const hhg_db* db) { return db ? db->total_cols : 0; }
 int hhg_db_lengths(const hhg_db* db, int32_t* out) {
   if (!db || !out) return fail(HHG_EINVAL, "hhg_db_lengths: bad argument");
   memcpy(out, db->L.data(), (size_t)db->n * sizeof(int32_t));
+  return HHG_OK;
+}
+
+
+// ------------------------------------------------------------------------- host-resident store + staged shard
+// HHEntry::getTemplateHMM reads only the prefilter's survivors (src/hhdatabase.cpp:300-336); here the records of all
+// profiles sit in page-locked host memory and hhg_db_stage brings the survivors into a device cache (DESIGN 4.12).
+int hhg_dbstore_create(hhg_ctx* ctx, int capacity_targets, long long capacity_cols, int has_ss, hhg_dbstore** out) {
+  if (!ctx || !out || capacity_targets < 1 || capacity_cols < capacity_targets)
+    return fail(HHG_EINVAL, "hhg_dbstore_create: bad argument (every target has at least one column)");
+  CK(cudaSetDevice(ctx->device));
+  std::unique_ptr<hhg_dbstore> st(new hhg_dbstore());
+  st->device = ctx->device;
+  st->has_ss = has_ss != 0;
+  st->cap_targets = capacity_targets;
+  st->cap_cols = capacity_cols;
+  const unsigned flags = cudaHostAllocMapped | cudaHostAllocPortable;
+  cudaError_t e1 = cudaHostAlloc((void**)&st->cols, (size_t)capacity_cols * sizeof(ColRec), flags);
+  cudaError_t e2 = e1 == cudaSuccess ? cudaHostAlloc((void**)&st->pav, (size_t)capacity_targets * 80, flags) : e1;
+  if (e2 != cudaSuccess) {
+    if (e1 == cudaSuccess) cudaFreeHost(st->cols);
+    cudaGetLastError();
+    return fail(HHG_ENOMEM, "hhg_dbstore_create: cannot page-lock %.3f GB of host memory (%s)",
+                ((double)capacity_cols * sizeof(ColRec) + (double)capacity_targets * 80) / 1e9, cudaGetErrorString(e2));
+  }
+  void *dc = nullptr, *dp = nullptr;
+  cudaError_t e3 = cudaHostGetDevicePointer(&dc, st->cols, 0), e4 = cudaHostGetDevicePointer(&dp, st->pav, 0);
+  if (e3 != cudaSuccess || e4 != cudaSuccess) {
+    cudaFreeHost(st->cols); cudaFreeHost(st->pav);
+    return fail(HHG_ECUDA, "hhg_dbstore_create: the device cannot map host memory");
+  }
+  st->d_cols = (const float4*)dc;
+  st->d_pav = (const float*)dp;
+  *out = st.release();
+  return HHG_OK;
+}
+
+int hhg_dbstore_destroy(hhg_dbstore* store) {
+  if (!store) return HHG_OK;
+  if (store->users > 0) return fail(HHG_EINVAL, "hhg_dbstore_destroy: %d staged shards still use the store", store->users);
+  cudaSetDevice(store->device);
+  cudaFreeHost(store->cols);
+  cudaFreeHost(store->pav);
+  delete store;
+  return HHG_OK;
+}
+int hhg_dbstore_size(const hhg_dbstore* store) { return store ? store->n : 0; }
+long long hhg_dbstore_columns(const hhg_dbstore* store) { return store ? store->total_cols : 0; }
+int hhg_dbstore_lengths(const hhg_dbstore* store, int32_t* out) {
+  if (!store || !out) return fail(HHG_EINVAL, "hhg_dbstore_lengths: bad argument");
+  memcpy(out, store->L.data(), (size_t)store->n * sizeof(int32_t));
+  return HHG_OK;
+}
+
+// Checks that n more targets of lengths L fit and enters them in the store's tables; the caller then fills the records
+// [first, first + sum(L)) and pav rows [n0, n0 + n).  Nothing changes when it fails.
+static int dbstore_reserve(hhg_dbstore* st, const char* who, int n, const int32_t* L, long long* first) {
+  long long cols = 0;
+  for (int k = 0; k < n; ++k) {
+    if (L[k] < 1 || L[k] > 32767) return fail(HHG_EINVAL, "%s: target %d: length %d out of [1,32767]", who, k, L[k]);
+    cols += L[k];
+  }
+  if (st->n + (long long)n > st->cap_targets || st->total_cols + cols > st->cap_cols)
+    return fail(HHG_EINVAL, "%s: %lld targets / %lld columns needed, the store was created for %d / %lld", who,
+                st->n + (long long)n, st->total_cols + cols, st->cap_targets, st->cap_cols);
+  *first = st->total_cols;
+  for (int k = 0; k < n; ++k) {
+    st->L.push_back(L[k]);
+    st->col_off.push_back(st->total_cols);
+    st->total_cols += L[k];
+  }
+  st->n += n;
+  return HHG_OK;
+}
+
+int hhg_dbstore_append_packed(hhg_dbstore* store, int n, const int32_t* L, const void* cols_raw, const float* pav) {
+  if (!store || n < 1 || !L || !cols_raw || !pav) return fail(HHG_EINVAL, "hhg_dbstore_append_packed: bad argument");
+  const int n0 = store->n;
+  long long first = 0;
+  int rc = dbstore_reserve(store, "hhg_dbstore_append_packed", n, L, &first);
+  if (rc != HHG_OK) return rc;
+  memcpy(store->cols + first, cols_raw, (size_t)(store->total_cols - first) * sizeof(ColRec));
+  memcpy(store->pav + (size_t)n0 * 20, pav, (size_t)n * 80);
+  return HHG_OK;
+}
+
+int hhg_dbstore_append_db(hhg_ctx* ctx, hhg_dbstore* store, const hhg_db* db) {
+  if (!ctx || !store || !db) return fail(HHG_EINVAL, "hhg_dbstore_append_db: bad argument");
+  if (!db->raw || db->stage) return fail(HHG_EINVAL, "hhg_dbstore_append_db: the shard must be raw and not staged");
+  if (db->has_ss != store->has_ss) return fail(HHG_EINVAL, "hhg_dbstore_append_db: shard and store differ in has_ss");
+  if (db->device != ctx->device) return fail(HHG_EINVAL, "db lives on device %d, ctx on %d", db->device, ctx->device);
+  const int n0 = store->n;
+  long long first = 0;
+  int rc = dbstore_reserve(store, "hhg_dbstore_append_db", db->n, db->L.data(), &first);
+  if (rc != HHG_OK) return rc;
+  CK(cudaSetDevice(ctx->device));
+  CK(cudaMemcpyAsync(store->cols + first, db->cols_raw.p, (size_t)db->total_cols * sizeof(ColRec), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(store->pav + (size_t)n0 * 20, db->pav.p, (size_t)db->n * 80, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return HHG_OK;
+}
+
+int hhg_db_create_staged(hhg_ctx* ctx, hhg_dbstore* store, int max_targets, long long max_cols, hhg_db** out) {
+  if (!ctx || !store || !out || max_targets < 1 || max_cols < 1) return fail(HHG_EINVAL, "hhg_db_create_staged: bad argument");
+  if (store->device != ctx->device)
+    return fail(HHG_EINVAL, "hhg_db_create_staged: the store is mapped for device %d, ctx is on %d", store->device, ctx->device);
+  CK(cudaSetDevice(ctx->device));
+  std::unique_ptr<hhg_db> db(new hhg_db());
+  db->device = ctx->device;
+  db->n = max_targets;
+  db->total_cols = max_cols;
+  db->has_ss = store->has_ss;
+  db->L.assign(max_targets, 0);
+  db->col_off.assign(max_targets, 0);
+  db->raw = true;
+  db->prepared = false;
+  CK(db->cols.alloc((size_t)max_cols * 7));
+  CK(db->cols_raw.alloc((size_t)max_cols * 7));
+  CK(db->pav.alloc((size_t)max_targets * 20));
+  CK(db->dL.alloc(max_targets));
+  CK(db->dcol_off.alloc(max_targets));
+  CK(db->d_slot_id.alloc(max_targets));
+  CK(db->d_zero.alloc(max_targets));
+  std::vector<int> ident(max_targets);
+  std::iota(ident.begin(), ident.end(), 0);
+  CK(cudaMemcpyAsync(db->d_slot_id.p, ident.data(), (size_t)max_targets * 4, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemsetAsync(db->d_zero.p, 0, (size_t)max_targets * 4, ctx->stream));
+  CK(cudaMemsetAsync(db->dL.p, 0, (size_t)max_targets * 4, ctx->stream));
+  CK(cudaMemsetAsync(db->dcol_off.p, 0, (size_t)max_targets * 8, ctx->stream));
+  CK(cudaMemsetAsync(db->pav.p, 0, (size_t)max_targets * 80, ctx->stream));
+  CK(cudaMemsetAsync(db->cols_raw.p, 0, (size_t)max_cols * sizeof(ColRec), ctx->stream));
+  CK(cudaMemsetAsync(db->cols.p, 0, (size_t)max_cols * sizeof(ColRec), ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  db->stage.reset(new StageCache(max_targets, max_cols));
+  db->store = store;
+  store->users++;
+  *out = db.release();
+  return HHG_OK;
+}
+
+// CTAs of k_stage_gather: 8 warps each with 3.5 KB of loads in flight; 32 CTAs hold ~0.9 MB, several times the
+// bandwidth-delay product of a PCIe 5 x16 link (DESIGN 4.12 has the sweep).  HHG_STAGE_CTAS: developer knob of that sweep.
+static int stage_ctas() {
+  const char* e = getenv("HHG_STAGE_CTAS");
+  const int x = e ? atoi(e) : 0;
+  return x > 0 ? x : 32;
+}
+
+int hhg_db_stage(hhg_ctx* ctx, hhg_db* db, int n, const int32_t* global_ids, int32_t* local_ids_out,
+                 hhg_stage_stats* stats_out) {
+  if (!ctx || !db || n < 0 || (n && (!global_ids || !local_ids_out))) return fail(HHG_EINVAL, "hhg_db_stage: bad argument");
+  if (!db->stage) return fail(HHG_EINVAL, "hhg_db_stage: the shard was not made by hhg_db_create_staged");
+  if (db->device != ctx->device) return fail(HHG_EINVAL, "db lives on device %d, ctx on %d", db->device, ctx->device);
+  const hhg_dbstore* st = db->store;
+  std::vector<StageItem> items;
+  std::vector<int> freed;
+  StageStats ss{};
+  int bad = 0;
+  long long need_slots = 0, need_cols = 0;
+  const int rc = db->stage->request(n, global_ids, st->n, st->L.data(), st->col_off.data(), local_ids_out, &items, &freed,
+                                    &ss, &bad, &need_slots, &need_cols);
+  if (rc == -1) return fail(HHG_EINVAL, "hhg_db_stage: request %d: target id %d outside the store (%d targets)", bad, global_ids[bad], st->n);
+  if (rc == -2)
+    return fail(HHG_EINVAL, "hhg_db_stage: the request needs %lld slots and %lld columns, the staged shard has %d and %lld",
+                need_slots, need_cols, db->n, db->total_cols);
+  static_assert(sizeof(hhg_stage_stats) == sizeof(StageStats), "hhg_stage_stats layout");
+  if (stats_out) memcpy(stats_out, &ss, sizeof ss);
+  if (items.empty() && freed.empty()) return HHG_OK;
+  // one descriptor per copied target, then one per slot that only lost its target; run0 = first work item
+  std::vector<StageDesc> desc;
+  desc.reserve(items.size() + freed.size());
+  long long runs = 0;
+  for (const StageItem& it : items) {
+    desc.push_back(StageDesc{it.src, it.dst, it.len, it.slot, it.global, (int)runs});
+    runs += (it.len + kStageRun - 1) / kStageRun;
+    db->L[it.slot] = it.len;
+    db->col_off[it.slot] = it.dst;
+  }
+  for (int s : freed) {
+    desc.push_back(StageDesc{0, 0, 0, s, 0, (int)runs});
+    db->L[s] = 0;
+  }
+  // every plan over this shard describes the old slots: a new identity makes plan_build start over and hhg_plan_run
+  // refuse; `cols` no longer holds the null model of the new records
+  db->serial = g_db_serial.fetch_add(1);
+  db->cols_version++;
+  db->prepared = false;
+  CK(cudaSetDevice(ctx->device));
+  int arc = ctx_aux_stream(ctx);
+  if (arc != HHG_OK) return arc;
+  CK(db->d_desc.ensure(desc.size()));
+  // work already queued on the context stream may read the records this call overwrites, and may still read the
+  // descriptor buffer's last content: the gather starts after it, and the context stream goes on after the gather
+  CK(cudaEventRecord(ctx->aux_ev[0], ctx->stream));
+  CK(cudaStreamWaitEvent(ctx->aux_stream, ctx->aux_ev[0], 0));
+  CK(cudaMemcpyAsync(db->d_desc.p, desc.data(), desc.size() * sizeof(StageDesc), cudaMemcpyHostToDevice, ctx->aux_stream));
+  const int ctas = (int)std::max(1LL, std::min<long long>(stage_ctas(), std::max<long long>((runs + 7) / 8, ((long long)desc.size() + 31) / 32)));
+  k_stage_gather<<<ctas, 256, 0, ctx->aux_stream>>>((int)desc.size(), (int)runs, db->d_desc.p, st->d_cols, st->d_pav,
+                                                    db->cols_raw.p, db->pav.p, db->dL.p, db->dcol_off.p);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(ctx->aux_ev[1], ctx->aux_stream));
+  CK(cudaStreamWaitEvent(ctx->stream, ctx->aux_ev[1], 0));
+  return HHG_OK;
+}
+
+int hhg_db_staged_lookup(const hhg_db* db, int n, const int32_t* local_ids, int32_t* global_ids_out, int64_t* first_col_out) {
+  if (!db || !db->stage || n < 0 || (n && !local_ids)) return fail(HHG_EINVAL, "hhg_db_staged_lookup: bad argument / shard not staged");
+  for (int k = 0; k < n; ++k) {
+    const int s = local_ids[k];
+    if (s < 0 || s >= db->n) return fail(HHG_EINVAL, "hhg_db_staged_lookup: local id %d out of range", s);
+    if (global_ids_out) global_ids_out[k] = db->stage->global_of(s);
+    if (first_col_out) first_col_out[k] = db->stage->off_of(s);
+  }
   return HHG_OK;
 }
 
@@ -1543,6 +1804,7 @@ static int plan_build(hhg_ctx* ctx, hhg_plan* pl, const hhg_db* db, int n, const
   for (int k = 0; k < n; ++k) {
     const int id = ids ? ids[k] : k;
     if (id < 0 || id >= db->n) return fail(HHG_EINVAL, "request %d: target id %d out of range", k, id);
+    if (db->L[id] < 1) return fail(HHG_EINVAL, "request %d: slot %d of the staged shard is empty", k, id);
     const int q = req_query ? req_query[k] : 0;
     if (q < 0 || q >= ctx->nq) return fail(HHG_EINVAL, "request %d: query index %d out of range (batch of %d)", k, q, ctx->nq);
     pl->ids[k] = id; pl->req_query[k] = q;
@@ -1785,6 +2047,7 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
   if (!pl->built) return fail(HHG_EINVAL, "hhg_plan_run: the plan's last build failed");
   if (pl->q_L != ctx->q_L || pl->q_row0 != ctx->q_row0) return fail(HHG_EINVAL, "plan was made for another query (batch) geometry");
   const hhg_db* db = pl->db;
+  if (pl->db_serial != db->serial) return fail(HHG_EINVAL, "hhg_plan_run: the shard was staged anew after the plan was made");
   const bool fused = pl->nm_mode >= 0;     // null model factored in per job while the operand stream is built
   if (fused && (!db->raw || !ctx->has_q_pav)) return fail(HHG_EINVAL, "fused null model needs a raw shard and query pav");
   if (!fused && !db->prepared) return fail(HHG_EINVAL, "raw db: call hhg_db_apply_null_model for the current query first");
@@ -2271,6 +2534,7 @@ static int mac_realign_impl(hhg_ctx* ctx, const hhg_db* db, bool batch, int n, c
     if (q < 0 || q >= ctx->mac_nq) return fail(HHG_EINVAL, "%s: request %d: query index %d out of range (%d queries)", who, r, q, ctx->mac_nq);
     const int t = target[r];
     if (t < 0 || t >= db->n) return fail(HHG_EINVAL, "request %d: target id %d out of range", r, t);
+    if (db->L[t] < 1) return fail(HHG_EINVAL, "request %d: slot %d of the staged shard is empty", r, t);
     const int L = db->L[t], Lq = ctx->mac_qL[q];
     const int32_t* v = vit + (size_t)r * 5;
     const long long ns = vit_off[r + 1] - vit_off[r];
@@ -2469,11 +2733,8 @@ static int mac_realign_impl(hhg_ctx* ctx, const hhg_db* db, bool batch, int n, c
       map.insert(map.end(), large_ids.begin(), large_ids.end());
       int* d_map = ctx->mac_map.p + w0;
       CK(cudaMemcpyAsync(d_map, map.data(), map.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-      if (!ctx->aux_stream) {
-        CK(cudaStreamCreateWithFlags(&ctx->aux_stream, cudaStreamNonBlocking));
-        CK(cudaEventCreateWithFlags(&ctx->aux_ev[0], cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&ctx->aux_ev[1], cudaEventDisableTiming));
-      }
+      int arc = ctx_aux_stream(ctx);
+      if (arc != HHG_OK) return arc;
       CK(cudaEventRecord(ctx->aux_ev[0], ctx->stream));              // band + inputs ready
       CK(cudaStreamWaitEvent(ctx->aux_stream, ctx->aux_ev[0], 0));
       MacArgs AL = A;

@@ -768,6 +768,69 @@ __global__ void k_mac_gather_cols(int n, const int* __restrict__ req_q, const in
   }
 }
 
+// Staging of a host-resident store's targets into a staged shard (hhg_db_stage): descriptor d copies the len records
+// at store record src to arena record dst and fills slot's entries of L, col_off and pav; len == 0 marks a slot that
+// lost its target (only L is cleared).  `store` and `store_pav` are device-mapped page-locked HOST memory, so every
+// load crosses the PCIe link: latency, not SM throughput, bounds the copy.  A work item is one run of kStageRun records
+// of one target (a target's records are contiguous on both sides, a long target is several items, the last one short);
+// a warp takes an item, finds its target by bisection over run0 (first item of each descriptor) and every lane issues
+// its kStageRun * 7 / 32 independent 16-byte loads -- read once, so they bypass L1 -- before its first store.  A few
+// dozen warps keep more bytes in flight than the link's bandwidth-delay product, so the grid is small and the kernel
+// can share the device with a search running on another stream.
+constexpr int kStageRun = 32;                      // records per work item: 3584 B, 7 x 16 B per lane
+struct __align__(16) StageDesc {
+  long long src, dst;
+  int len, slot, global, run0;
+};
+static_assert(sizeof(StageDesc) == 32, "StageDesc is two 16-byte words");
+
+__device__ __forceinline__ float4 ld_stream(const float4* p) {
+  float4 v;
+  asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
+  return v;
+}
+
+__global__ void __launch_bounds__(256)
+k_stage_gather(int n_desc, int n_runs, const StageDesc* __restrict__ desc, const float4* __restrict__ store,
+               const float* __restrict__ store_pav, float4* __restrict__ cols_raw, float* __restrict__ pav,
+               int* __restrict__ L, long long* __restrict__ col_off) {
+  constexpr int kPer = kStageRun * 7 / 32;
+  const int lane = threadIdx.x & 31;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (int run = warp; run < n_runs; run += nwarps) {
+    int lo = 0, hi = n_desc - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (desc[mid].run0 <= run) lo = mid; else hi = mid - 1;
+    }
+    const StageDesc d = desc[lo];
+    const int r0 = (run - d.run0) * kStageRun;
+    const int nvec = min(kStageRun, d.len - r0) * 7;
+    const float4* src = store + (size_t)(d.src + r0) * 7;
+    float4* dst = cols_raw + (size_t)(d.dst + r0) * 7;
+    float4 v[kPer];
+#pragma unroll
+    for (int k = 0; k < kPer; ++k)
+      if (lane + 32 * k < nvec) v[k] = ld_stream(src + lane + 32 * k);
+#pragma unroll
+    for (int k = 0; k < kPer; ++k)
+      if (lane + 32 * k < nvec) dst[lane + 32 * k] = v[k];
+  }
+  // per-target entries: 5 lanes per descriptor move the 20 floats of pav, the first also writes L and col_off
+  for (int w = blockIdx.x * blockDim.x + threadIdx.x; w < n_desc * 8; w += gridDim.x * blockDim.x) {
+    const StageDesc d = desc[w >> 3];
+    const int part = w & 7;
+    if (part == 0) {
+      L[d.slot] = d.len;
+      if (d.len) col_off[d.slot] = d.dst;
+    }
+    if (d.len && part < 5)
+      reinterpret_cast<float4*>(pav + (size_t)d.slot * 20)[part] =
+          ld_stream(reinterpret_cast<const float4*>(store_pav + (size_t)d.global * 20) + part);
+  }
+}
+
 // Compact the per-request path strings (capacity Lq+Lt+2 each) to their real lengths before the D2H copy:
 // one thread per request copies nsteps bytes to its compact offset.
 __global__ void k_gather_paths(int n, const HitRec* hits, const ReqDesc* reqs, const long long* dst_off,

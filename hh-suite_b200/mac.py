@@ -99,3 +99,14 @@ def realign_batch(ctx: capi.Context, db: capi.TargetDB, queries, hits, q_pav=Non
                 alt[(q, t)][0].append(int(m.i[0]) if len(m.i) else m.i2); alt[(q, t)][1].append(int(m.j[0]) if len(m.j) else m.j2)
         rnd += 1
     return out
+
+
+def to_global(db: capi.StagedDB, results: dict) -> dict:
+    """The results of realign / one query's results of realign_batch over a staged shard (hits with LOCAL targets, all
+    still resident), re-keyed and relabelled with the store's global ids.  Call before the next db.stage()."""
+    g = db.to_global([t for t, _ in results])
+    out = {}
+    for (_, irep), t, m in zip(results, g, results.values()):
+        m.target = int(t)
+        out[(int(t), irep)] = m
+    return out

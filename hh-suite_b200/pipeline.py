@@ -3,6 +3,8 @@ prefilter over the whole shard, then Viterbi (with alternative alignments) on th
 Everything between the stages is the reference's selection logic (prefilter.py, runner.py)."""
 from __future__ import annotations
 
+import dataclasses
+
 import numpy as np
 
 from . import capi, prefilter, runner
@@ -46,6 +48,55 @@ def search_batch(ctx: capi.Context, db: capi.TargetDB, csdb: capi.CsDB, queries,
     hits = runner.BatchViterbiRunner(ctx, db, altali=altali, smin=smin).alignment(rq, np.concatenate(ids)) \
         if len(rq) else [[] for _ in queries]
     return list(zip(ids, hits))
+
+
+def search_staged(ctx: capi.Context, db: capi.StagedDB, csdb: capi.CsDB, q_p, q_tr, q_pav, lib219, q_prefilter_p=None,
+                  altali=4, smin=20.0, cs_names=None, db_names=None, columnscore=1, pb=None, **pf_kwargs):
+    """search() over a database whose profiles stay in host memory (db.store): the prefilter's survivors are staged
+    into db (one hhg_db_stage call), the query's null model is applied to the staged records (columnscore / pb as in
+    TargetDB.apply_null_model) and the same runner aligns them.  Returns what search() returns over a resident raw shard
+    of the whole database after apply_null_model(q_pav, pb, columnscore): survivor ids and Hit.target are GLOBAL ids.
+    The survivors of one query must fit db (HhgError otherwise, with the sizes needed)."""
+    prof = capi.build_prefilter_profile(q_p if q_prefilter_p is None else q_prefilter_p, q_pav, lib219,
+                                        pf_kwargs.get("score_offset", 50), pf_kwargs.get("bit_factor", 4))
+    ids = _to_targets(prefilter.prefilter_db(csdb, prof, **pf_kwargs), db.store, csdb, cs_names, db_names)
+    if not len(ids):
+        return ids, []
+    local = db.stage(ids)
+    db.apply_null_model(q_pav, pb, columnscore)
+    ctx.set_query(q_p, q_tr)
+    hits = runner.ViterbiRunner(ctx, db, altali=altali, smin=smin).alignment(local)
+    return ids, to_global_hits(db, hits)
+
+
+def search_batch_staged(ctx: capi.Context, db: capi.StagedDB, csdb: capi.CsDB, queries, lib219, altali=4, smin=20.0,
+                        cs_names=None, db_names=None, columnscore=1, pb=None, **pf_kwargs):
+    """search_batch() over a database whose profiles stay in host memory: the union of all queries' survivors is staged
+    in one call, then the batch runner aligns every query with its own survivors, the null model of each query fused
+    into the search (so q_pav of every query is used: pass (q_p, q_tr, q_pav[, q_prefilter_p]) as for search_batch).
+    Returns what search_batch() returns over a resident raw shard of the whole database, with GLOBAL ids.  The union
+    must fit db."""
+    so, bf = pf_kwargs.get("score_offset", 50), pf_kwargs.get("bit_factor", 4)
+    profs = [capi.build_prefilter_profile(q[0] if len(q) < 4 or q[3] is None else q[3], q[2], lib219, so, bf)
+             for q in queries]
+    ids = [_to_targets(x, db.store, csdb, cs_names, db_names)
+           for x in prefilter.prefilter_db_batch(csdb, profs, **pf_kwargs)]
+    rq = np.concatenate([np.full(len(x), q, np.int32) for q, x in enumerate(ids)])
+    if not len(rq):
+        return [(x, []) for x in ids]
+    local = db.stage(np.concatenate(ids))
+    capi.query_set_batch(ctx, [(q[0], q[1]) for q in queries], q_pav=np.stack([q[2] for q in queries]))
+    hits = runner.BatchViterbiRunner(ctx, db, altali=altali, smin=smin, columnscore=columnscore, pb=pb).alignment(rq, local)
+    return [(x, to_global_hits(db, h)) for x, h in zip(ids, hits)]
+
+
+def to_global_hits(db: capi.StagedDB, hits):
+    """Hits of a search over a staged shard with Hit.target translated from local to global ids (new objects; use
+    before the next stage() call, and give mac.realign the LOCAL hits)."""
+    if not hits:
+        return []
+    g = db.to_global([h.target for h in hits])
+    return [dataclasses.replace(h, target=int(t)) for h, t in zip(hits, g)]
 
 
 def _to_targets(ids, db, csdb, cs_names, db_names):

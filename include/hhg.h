@@ -17,6 +17,7 @@
  *   Prefilter::swStripedByte            src/hhprefilter.h:112      -> hhg_prefilter_sw
  *   HHEntry::getTemplateHMM / HMM::Read src/hhdatabase.cpp:300, src/hhhmm.cpp:202 -> hhg_db_create_hhm
  *   PrepareTemplateHMM                  src/hhfunc.cpp:165         -> hhg_db_create_hhm + hhg_db_apply_null_model
+ *   HHEntry::getTemplateHMM, survivors  src/hhdatabase.cpp:300, src/hhprefilter.cpp:561 -> hhg_dbstore_create + hhg_db_stage
  *   PosteriorDecoder::realign           src/hhposteriordecoder.h:67 -> hhg_mac_realign
  *   PosteriorDecoderRunner (hhblits_omp, one per query)               -> hhg_mac_realign_batch
  *
@@ -283,6 +284,60 @@ int hhg_db_destroy(hhg_db* db);
 int hhg_db_size(const hhg_db* db);          /* number of targets */
 long long hhg_db_columns(const hhg_db* db); /* sum of target lengths */
 int hhg_db_lengths(const hhg_db* db, int32_t* out /* [hhg_db_size] */);
+
+/* ---- databases larger than device memory: a host-resident profile store and a staged shard ------------------------
+ * The reference never holds the profile database in memory: Prefilter::prefilter_db hands the NAMES of its survivors on
+ * (src/hhprefilter.cpp:561-590) and HHEntry::getTemplateHMM (src/hhdatabase.cpp:300-336) reads only those entries from
+ * the mmap'd ffindex.  Here the cs219 shard (one byte per column) stays on the device, the 112-byte column records of
+ * all profiles stay in page-locked, device-mapped HOST memory (hhg_dbstore), and a staged shard is a device cache over
+ * them that holds each query's or query batch's survivors.
+ *
+ * hhg_dbstore_create: room for capacity_targets targets and capacity_cols columns (112 bytes each, plus 80 bytes of
+ *   pav per target), allocated at once and page-locked; has_ss as in hhg_db_create_packed.
+ * hhg_dbstore_append_packed: n more targets from host arrays in the format hhg_db_read_cols with which = 0 and
+ *   hhg_db_read_pav write (lengths L[n], sum(L) records, pav[n*20]).
+ * hhg_dbstore_append_db: all targets of a raw device shard (hhg_db_create_raw / _hhm / _a3m / _ca3m / _packed), so a
+ *   database of any format is loaded chunk by chunk: create a shard of one chunk, append it, destroy it.
+ * Both refuse, before anything is copied, what does not fit the capacity, a length outside [1, 32767], a shard whose
+ * has_ss differs from the store's, and a shard that is not raw or is itself staged.  Targets are numbered in append
+ * order: these are the GLOBAL ids.  A store is destroyed after the staged shards made over it. */
+typedef struct hhg_dbstore hhg_dbstore;
+int hhg_dbstore_create(hhg_ctx* ctx, int capacity_targets, long long capacity_cols, int has_ss, hhg_dbstore** out);
+int hhg_dbstore_append_packed(hhg_dbstore* store, int n, const int32_t* L, const void* cols_raw, const float* pav);
+int hhg_dbstore_append_db(hhg_ctx* ctx, hhg_dbstore* store, const hhg_db* db);
+int hhg_dbstore_destroy(hhg_dbstore* store);
+int hhg_dbstore_size(const hhg_dbstore* store);          /* number of targets appended */
+long long hhg_dbstore_columns(const hhg_dbstore* store); /* sum of their lengths */
+int hhg_dbstore_lengths(const hhg_dbstore* store, int32_t* out /* [hhg_dbstore_size] */);
+/* hhg_db_create_staged: a raw shard of max_targets slots over an arena of max_cols columns, empty at first.  It is an
+ *   hhg_db: hhg_viterbi_search(_batch), hhg_plan_create, hhg_db_apply_null_model, hhg_mac_realign(_batch) and the
+ *   read_* calls take it with LOCAL ids = slots (hhg_db_size is max_targets, hhg_db_columns is max_cols, an empty
+ *   slot has length 0 and is refused as a target).  The store must live on ctx's device.
+ * hhg_db_stage: makes the n targets global_ids[] resident and writes their local ids to local_ids_out[n] (duplicates
+ *   share a slot).  Resident targets keep their local id and are not copied.  Missing ones take free slots and free
+ *   arena runs; when there is none, targets this call does not name are evicted, least recently staged first, until a
+ *   run fits.  The records of all missing targets arrive in ONE kernel launch that reads the store through its
+ *   device-mapped pointer, on the context's auxiliary stream; the context stream waits for it by event, the host does
+ *   not.  After a call that copied or evicted anything the shard is as after hhg_db_create_packed (apply the null
+ *   model again before a single-query search), earlier local ids of evicted targets are void, the context's search
+ *   plan is rebuilt and an hhg_plan made before the call refuses to run; a call that found everything resident
+ *   changes nothing.
+ *   A call whose distinct targets need more slots or columns than the shard has is HHG_EINVAL (the message gives
+ *   both numbers), as is an id outside the store; the shard is then unchanged.
+ *   stats_out (may be NULL): what this call did.
+ * hhg_db_staged_lookup: global id (-1 for an empty slot) and first arena column (the `first` of hhg_db_read_cols) of
+ *   n local ids; either output may be NULL. */
+typedef struct hhg_stage_stats {
+  int64_t hits;      /* distinct targets that were already resident */
+  int64_t copied;    /* distinct targets copied from the store       */
+  int64_t bytes;     /* bytes written to the device for them         */
+  int64_t evicted;   /* targets that lost their slot                 */
+} hhg_stage_stats;
+int hhg_db_create_staged(hhg_ctx* ctx, hhg_dbstore* store, int max_targets, long long max_cols, hhg_db** out);
+int hhg_db_stage(hhg_ctx* ctx, hhg_db* db, int n, const int32_t* global_ids, int32_t* local_ids_out,
+                 hhg_stage_stats* stats_out);
+int hhg_db_staged_lookup(const hhg_db* db, int n, const int32_t* local_ids, int32_t* global_ids_out,
+                         int64_t* first_col_out);
 
 /* Set the query (replaces HMMSimd::MapOneHMM).  S33: float[44*44] or NULL (needed iff use_ss). */
 int hhg_query_set(hhg_ctx* ctx, int Lq, const float* p, const float* tr, const uint8_t* ss,
