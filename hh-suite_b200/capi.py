@@ -53,7 +53,8 @@ SYMBOLS = ["hhg_last_error", "hhg_ctx_create", "hhg_ctx_destroy", "hhg_ctx_sync"
            "hhg_prefilter_sw_batch", "hhg_prefilter_batch_max_queries",
            "hhg_dbstore_create", "hhg_dbstore_append_packed", "hhg_dbstore_append_db", "hhg_dbstore_destroy",
            "hhg_dbstore_size", "hhg_dbstore_columns", "hhg_dbstore_lengths", "hhg_db_create_staged", "hhg_db_stage",
-           "hhg_db_staged_lookup"]
+           "hhg_db_staged_lookup", "hhg_recsrc_create_hhm", "hhg_recsrc_create_a3m", "hhg_recsrc_create_ca3m",
+           "hhg_recsrc_destroy", "hhg_recsrc_size", "hhg_db_create_staged_records", "hhg_db_staged_neff"]
 
 
 class PrepParams(C.Structure):
@@ -365,6 +366,16 @@ def load():
     L.hhg_db_create_staged.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.POINTER(C.c_void_p)]
     L.hhg_db_stage.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, c_i32p, C.c_void_p]
     L.hhg_db_staged_lookup.argtypes = [C.c_void_p, C.c_int, c_i32p, c_i32p, c_i64p]
+    L.hhg_recsrc_create_hhm.argtypes = [C.c_void_p, C.c_int, C.c_char_p, c_i64p, c_i64p, C.POINTER(PrepParams), c_f32p,
+                                        C.c_int, C.POINTER(C.c_void_p)]
+    L.hhg_recsrc_create_a3m.argtypes = [C.c_void_p, C.c_int, C.c_char_p, c_i64p, c_i64p, C.c_void_p, c_f32p, c_f32p,
+                                        C.POINTER(PrepParams), c_f32p, C.c_int, C.POINTER(C.c_void_p)]
+    L.hhg_recsrc_create_ca3m.argtypes = [C.c_void_p, C.c_int, C.c_char_p, c_i64p, c_i64p, C.c_void_p, C.c_void_p, c_f32p,
+                                         c_f32p, C.POINTER(PrepParams), c_f32p, C.c_int, C.POINTER(C.c_void_p)]
+    L.hhg_recsrc_destroy.argtypes = [C.c_void_p]
+    L.hhg_recsrc_size.argtypes = [C.c_void_p]
+    L.hhg_db_create_staged_records.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.POINTER(C.c_void_p)]
+    L.hhg_db_staged_neff.argtypes = [C.c_void_p, C.c_int, c_i32p, c_f32p]
     _lib = L
     return L
 
@@ -850,17 +861,81 @@ class HostStore:
             self.h = None
 
 
+class RecordSource:
+    """A database's own ffindex records (HHM, A3M or compressed A3M) as what a StagedDB stages from (hhg_recsrc): no
+    record is parsed until a stage() call names it.  Global ids are record indices.  The data buffer (bytes or an mmap
+    of the ffdata) and the SeqDb are kept referenced here and must stay valid while the source lives."""
+
+    def __init__(self, ctx: Context, data: bytes, offsets, lengths, create, *args):
+        """Shared body of the from_* constructors: create(ctx, n, data, offsets, lengths, *args, out)."""
+        off = np.ascontiguousarray(offsets, np.int64); ln = np.ascontiguousarray(lengths, np.int64)
+        n = len(off)
+        if n == 0 or len(ln) != n or off.min() < 0 or ln.min() < 0 or int((off + ln).max()) > len(data):
+            raise ValueError("offsets/lengths do not fit the data buffer")
+        self.ctx, self._buf, self._off, self._len = ctx, np.frombuffer(data, np.uint8), off, ln
+        h = C.c_void_p()
+        _ck(create(ctx.h, n, self._buf.ctypes.data_as(C.c_char_p), _p(off, c_i64p), _p(ln, c_i64p), *args, C.byref(h)))
+        self.h = h
+
+    @classmethod
+    def from_hhm(cls, ctx, data: bytes, offsets, lengths, R, params: "PrepParams | None" = None, has_ss: bool = False):
+        """HHM records, with the arguments of TargetDB.from_hhm."""
+        R = np.ascontiguousarray(R, np.float32)
+        assert R.shape == (20, 20)
+        pp = params or PrepParams.defaults()
+        self = cls(ctx, data, offsets, lengths, ctx.L.hhg_recsrc_create_hhm, C.byref(pp), _p(R, c_f32p), 1 if has_ss else 0)
+        self._keep = (pp, R)
+        return self
+
+    @classmethod
+    def from_a3m(cls, ctx, data: bytes, offsets, lengths, R, pb, S=None, params: "PrepParams | None" = None,
+                 mp: "MsaParams | None" = None, has_ss: bool = False):
+        """A3M alignments, with the arguments of TargetDB.from_a3m."""
+        return cls._from_msa(ctx, data, offsets, lengths, None, R, pb, S, params, mp, has_ss)
+
+    @classmethod
+    def from_ca3m(cls, ctx, data: bytes, offsets, lengths, seqs: "SeqDb", R, pb, S=None,
+                  params: "PrepParams | None" = None, mp: "MsaParams | None" = None, has_ss: bool = False):
+        """Compressed alignments, with the arguments of TargetDB.from_ca3m."""
+        return cls._from_msa(ctx, data, offsets, lengths, seqs, R, pb, S, params, mp, has_ss)
+
+    @classmethod
+    def _from_msa(cls, ctx, data, offsets, lengths, seqs, R, pb, S, params, mp, has_ss):
+        R = np.ascontiguousarray(R, np.float32); pb = np.ascontiguousarray(pb, np.float32)
+        Sm = None if S is None else np.ascontiguousarray(S, np.float32)
+        pp = params or PrepParams.defaults()
+        mp = mp or MsaParams.defaults()
+        args = (C.byref(mp), _p(Sm, c_f32p), _p(pb, c_f32p), C.byref(pp), _p(R, c_f32p), 1 if has_ss else 0)
+        if seqs is None:
+            self = cls(ctx, data, offsets, lengths, ctx.L.hhg_recsrc_create_a3m, *args)
+        else:
+            self = cls(ctx, data, offsets, lengths, ctx.L.hhg_recsrc_create_ca3m, C.byref(seqs), *args)
+        self._keep = (seqs,)
+        return self
+
+    @property
+    def n(self) -> int:
+        return int(self.ctx.L.hhg_recsrc_size(self.h))
+
+    def close(self):
+        if self.h:
+            _ck(self.ctx.L.hhg_recsrc_destroy(self.h))
+            self.h = None
+
+
 STAGE_STATS_DTYPE = np.dtype([("hits", np.int64), ("copied", np.int64), ("bytes", np.int64), ("evicted", np.int64)])
 
 
 class StagedDB(TargetDB):
-    """A TargetDB of max_targets slots that caches targets of a HostStore (hhg_db_create_staged).  Every TargetDB use
-    works on it with LOCAL ids (slots); stage() makes targets resident, to_global() translates back.  n is the number
-    of slots, Lh the length of the target in each slot (0: empty)."""
+    """A TargetDB of max_targets slots that caches targets of a HostStore (hhg_db_create_staged) or builds them from a
+    RecordSource's records when they are staged (hhg_db_create_staged_records); `store` is the one it was made over.
+    Every TargetDB use works on it with LOCAL ids (slots); stage() makes targets resident, to_global() translates back.
+    n is the number of slots, Lh the length of the target in each slot (0: empty)."""
 
-    def __init__(self, ctx: Context, store: HostStore, max_targets: int, max_cols: int):
+    def __init__(self, ctx: Context, store: "HostStore | RecordSource", max_targets: int, max_cols: int):
         h = C.c_void_p()
-        _ck(ctx.L.hhg_db_create_staged(ctx.h, store.h, max_targets, max_cols, C.byref(h)))
+        create = ctx.L.hhg_db_create_staged_records if isinstance(store, RecordSource) else ctx.L.hhg_db_create_staged
+        _ck(create(ctx.h, store.h, max_targets, max_cols, C.byref(h)))
         self.ctx, self.h, self.n, self.store = ctx, h, max_targets, store
         self.Lh = np.zeros(max_targets, np.int32)
         self.last_stats = np.zeros(1, STAGE_STATS_DTYPE)[0]
@@ -889,6 +964,13 @@ class StagedDB(TargetDB):
     def read_target(self, local: int):
         """Raw column records of the target in slot `local`."""
         return self.read_cols(0, int(self.lookup([local])[1][0]), int(self.Lh[local]))
+
+    def neff(self, local) -> np.ndarray:
+        """Neff_HMM of the targets in slots `local` (record-sourced shards only): the t_neff of hitlist_pvalues."""
+        local = np.ascontiguousarray(local, np.int32)
+        out = np.zeros(len(local), np.float32)
+        _ck(self.ctx.L.hhg_db_staged_neff(self.h, len(local), _p(local, c_i32p), _p(out, c_f32p)))
+        return out
 
 
 class Comm:

@@ -30,6 +30,8 @@
 #include <numeric>
 #include <string>
 #include <thread>
+#include <type_traits>
+#include <unordered_set>
 #include <vector>
 
 using namespace hhg;
@@ -207,6 +209,23 @@ struct hhg_dbstore {
   int users = 0;                 // staged shards made over this store
 };
 
+// A database's own ffindex records as the source of a staged shard (hhg_recsrc_*): the record text stays the
+// caller's (typically an mmap of the ffdata); only offsets, lengths and parameters are copied.
+struct hhg_recsrc {
+  int device = 0;
+  int kind = 0;                     // 0 HHM, 1 A3M, 2 compressed A3M
+  int n = 0;
+  const char* data = nullptr;
+  std::vector<int64_t> off, len;
+  hhg_seqdb seqs{};                 // compressed A3M: the sequence database (its arrays stay the caller's)
+  hhg_msa_params mp{};
+  hhg_prep_params pp{};
+  std::vector<float> S, pb, R;      // S empty: not given
+  bool has_ss = false;
+  std::vector<int32_t> L;           // columns of each record, 0 until a stage call has scanned it
+  int users = 0;                    // staged shards made over this source
+};
+
 struct hhg_db {
   // identity for plan reuse (addresses get recycled); a staged shard takes a new one whenever hhg_db_stage changes a slot
   unsigned long long serial = g_db_serial.fetch_add(1);
@@ -229,6 +248,12 @@ struct hhg_db {
   std::unique_ptr<StageCache> stage;
   DevBuf<StageDesc> d_desc;
   DevBuf<int> d_slot_id, d_zero;         // 0..n-1 and zeros: k_mac_gather_cols' request arrays for a pass over all slots
+  // record-sourced staged shard (hhg_db_create_staged_records): targets are built from src's records
+  hhg_recsrc* src = nullptr;
+  std::shared_ptr<void> builder;         // the source's MsaBuilder / HhmBuilder, device buffers kept between calls
+  std::vector<float> neff;               // [n] Neff_HMM of the target in each slot
+  DevBuf<float4> rec_cols;               // one group's built records and pav rows: k_stage_gather's source
+  DevBuf<float> rec_pav;
 };
 
 struct hhg_csdb {
@@ -622,8 +647,9 @@ int msa_upload(hhg_ctx* ctx, DevBuf<T>& d, const std::vector<V>& h) {
   return HHG_OK;
 }
 
-// C.host is filled (parsed); runs the four kernels and leaves f / tr / Neff / keep / wg on the device.
-int msa_chunk_run(hhg_ctx* ctx, MsaChunk& C, const hhg_msa_params& mp, const float* S, const float* pb, int first_record) {
+// C.host is filled (parsed); runs the four kernels and leaves f / tr / Neff / keep / wg on the device.  An error names
+// alignment k by rec[k] (rec NULL: by k).
+int msa_chunk_run(hhg_ctx* ctx, MsaChunk& C, const hhg_msa_params& mp, const float* S, const float* pb, const int32_t* rec) {
   const int m = (int)C.host.size();
   C.desc.resize(m);
   C.seq_total = C.col_total = C.x_total = C.ins_total = 0;
@@ -731,7 +757,7 @@ int msa_chunk_run(hhg_ctx* ctx, MsaChunk& C, const hhg_msa_params& mp, const flo
   CK(cudaStreamSynchronize(ctx->stream));
   for (int k = 0; k < m; ++k)
     if (status[k])
-      return fail(HHG_EINVAL, "alignment %d: %s", first_record + k,
+      return fail(HHG_EINVAL, "alignment %d: %s", rec ? rec[k] : k,
                   status[k] == 1 ? "contains no sequences after filtering (the reference exits here)"
                   : status[k] == 2 ? "the position-dependent identity schedule divides by zero (as in the reference)"
                                    : "no sequence left for the profile");
@@ -897,7 +923,7 @@ static int msa_to_hmm_impl(hhg_ctx* ctx, const char* rec, int64_t len, const hhg
   const MsaHost& H = C.host[0];
   msa_dims(H, dims);
   if (H.L > L_cap || H.N_in > N_cap) return fail(HHG_EINVAL, "hhg_msa_to_hmm: %d columns / %d sequences exceed the caller's capacity %d / %d", H.L, H.N_in, L_cap, N_cap);
-  rc = msa_chunk_run(ctx, C, *mp, S, pb, 0);
+  rc = msa_chunk_run(ctx, C, *mp, S, pb, nullptr);
   if (rc != HHG_OK) return rc;
   const int L = H.L, N = H.N_in;
   int nf = 0;
@@ -938,75 +964,85 @@ int hhg_ca3m_scan(const char* rec, int64_t len, const hhg_seqdb* seqs, const hhg
   return HHG_OK;
 }
 
-static int db_create_a3m_impl(hhg_ctx* ctx, int n, const char* data, const int64_t* off, const int64_t* len,
-                              const hhg_seqdb* sq, const hhg_msa_params* mp, const float* S, const float* pb,
-                              const hhg_prep_params* pp, const float* R, hhg_db** out, float* d_tr_full,
-                              float* neff_hmm_out) {
-  if (!ctx || !out || n <= 0 || !data || !off || !len || !pp || !R || !pb)
-    return fail(HHG_EINVAL, "hhg_db_create_a3m: bad argument");
-  int rc = msa_params_check(mp);
-  if (rc != HHG_OK) return rc;
-  if ((rc = seqdb_check(sq)) != HHG_OK) return rc;
-  if (mp->qsc > -10.f && !S) return fail(HHG_EINVAL, "hhg_db_create_a3m: the qsc filter needs the substitution matrix S");
-  HhmPrepArgs A;
-  if ((rc = hhm_prep_args("hhg_db_create_a3m", pp, R, &A)) != HHG_OK) return rc;
-  const bool tau_on_host = pp->pcm == 2 && pp->pcc != 1.0f;
-  CK(cudaSetDevice(ctx->device));
-  const bool timing = getenv("HHG_TIMING") != nullptr;
-  const auto t_begin = std::chrono::steady_clock::now();
-  double ms_scan = 0.0, ms_kernels = 0.0;
+// The records of an ffindex: record r is the len[r] bytes at data + off[r].
+struct RecText {
+  const char* data;
+  const int64_t* off;
+  const int64_t* len;
+};
 
-  // The records go through in groups: host scan of a group (threads) -> kernels -> column records of the group in a
-  // device piece; the shard is assembled from the pieces at the end.  Host memory holds one group of parsed
-  // alignments at a time (a database of alignments is far larger than the shard it turns into).
-  struct Piece { DevBuf<float4> cols; DevBuf<float> pav; int first = 0, n = 0; long long ncols = 0; };
-  std::vector<std::unique_ptr<Piece>> pieces;
-  std::vector<int32_t> Ls(n);
-  long long tot = 0;
-  bool any_ss = false;
-
-  const long long kGroupText = 256ll << 20;           // bytes of input text per group
-  int max_records = 8192;
-  { const char* e = getenv("HHG_MSA_CHUNK_RECORDS"); if (e && atoi(e) > 0) max_records = atoi(e); }   // test knob: many small groups
+// Alignment records -> raw column records and pav, one group at a time: scan() parses a group on the host threads,
+// build() runs filter / weights / M state / finish, k_msa_prepare and k_hhm_pav and writes the group's records to dst
+// (in group order, each record's columns contiguous) and its pav rows to pav.  The A3M / CA3M shard loader and the
+// stage of a record-sourced shard (hhg_db_stage) both go through it; host memory holds one group of parsed alignments.
+struct MsaBuilder {
+  hhg_ctx* ctx = nullptr;
+  RecText T{};
+  const hhg_seqdb* sq = nullptr;       // non-NULL: compressed A3M
+  const hhg_msa_params* mp = nullptr;
+  const float* S = nullptr;
+  const float* pb = nullptr;
+  const hhg_prep_params* pp = nullptr;
+  HhmPrepArgs A{};
   MsaChunk C;
   DevBuf<long long> d_rec_off;
   DevBuf<uint8_t> d_ss;
   DevBuf<float> d_tau;
   DevBuf<int> d_L;
-  int t0 = 0;
-  while (t0 < n) {
-    int t1 = t0;
+  std::vector<int32_t> rec, L;         // the scanned group: record indices and their lengths
+  std::vector<long long> rec_off;      // first output column of each record of the group
+  long long cols = 0;
+  bool any_ss = false;                 // some record scanned so far predicts secondary structure
+
+  // end of the group that starts at r[k0] of r[0..n): 256 MB of input text or max_records records
+  int group_end(const int32_t* r, int k0, int n, const int32_t*) const {
+    const long long kGroupText = 256ll << 20;
+    int max_records = 8192;
+    { const char* e = getenv("HHG_MSA_CHUNK_RECORDS"); if (e && atoi(e) > 0) max_records = atoi(e); }   // test knob: many small groups
+    int k1 = k0;
     long long bytes = 0;
-    while (t1 < n && t1 - t0 < max_records && (bytes == 0 || bytes + len[t1] <= kGroupText)) bytes += len[t1++];
-    const int m = t1 - t0;
-    const auto t_s0 = std::chrono::steady_clock::now();
+    while (k1 < n && k1 - k0 < max_records && (bytes == 0 || bytes + T.len[r[k1]] <= kGroupText)) bytes += T.len[r[k1++]];
+    return k1;
+  }
+  // the lengths come from the full parse of scan()
+  int peek(const int32_t*, int, int32_t*) { return HHG_OK; }
+
+  int scan(const int32_t* r, int m) {
+    rec.clear();
     C.host.clear();
     C.host.resize(m);
     const HostFail bad = host_for(m, [&](int k) -> std::string {
-      if (len[t0 + k] <= 0) return "empty record";
-      return msa_parse_any(data + off[t0 + k], len[t0 + k], sq, mp, &C.host[k]);
+      if (T.len[r[k]] <= 0) return "empty record";
+      return msa_parse_any(T.data + T.off[r[k]], T.len[r[k]], sq, mp, &C.host[k]);
     });
-    if (bad.k >= 0) return fail(HHG_EINVAL, "record %d: %s", t0 + bad.k, bad.msg.c_str());
-    std::vector<long long> rec_off(m);
-    long long cols = 0;
+    if (bad.k >= 0) return fail(HHG_EINVAL, "record %d: %s", r[bad.k], bad.msg.c_str());
+    L.resize(m);
+    rec_off.resize(m);
+    cols = 0;
     for (int k = 0; k < m; ++k) {
-      const int L = C.host[k].L;
-      if (L > 32767) return fail(HHG_EINVAL, "record %d: length %d out of [1,32767]", t0 + k, L);
-      Ls[t0 + k] = L;
-      rec_off[k] = cols; cols += L;
+      const int Lk = C.host[k].L;
+      if (Lk < 1 || Lk > 32767) return fail(HHG_EINVAL, "record %d: length %d out of [1,32767]", r[k], Lk);
+      L[k] = Lk;
+      rec_off[k] = cols; cols += Lk;
       any_ss |= C.host[k].kss_pred >= 0;
     }
-    ms_scan += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_s0).count();
-    const auto t_c0 = std::chrono::steady_clock::now();
-    rc = msa_chunk_run(ctx, C, *mp, S, pb, t0);
+    rec.assign(r, r + m);
+    return HHG_OK;
+  }
+
+  // ss: write the ss bytes of the records (else 0); d_tr_full: hhg_query_from_a3m's linear transitions (one record);
+  // neff_out: Neff_HMM of each record (host)
+  int build(bool ss, ColRec* dst, float* pav, float* d_tr_full, float* neff_out) {
+    const int m = (int)rec.size();
+    const bool tau_on_host = pp->pcm == 2 && pp->pcc != 1.0f;
+    int rc = msa_chunk_run(ctx, C, *mp, S, pb, rec.data());
     if (rc != HHG_OK) return rc;
-    ms_kernels += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_c0).count();
     std::vector<uint8_t> ssb((size_t)cols, 0);
-    for (int k = 0; k < m; ++k) msa_ss_bytes(C.host[k], ssb.data() + rec_off[k]);
+    if (ss) for (int k = 0; k < m; ++k) msa_ss_bytes(C.host[k], ssb.data() + rec_off[k]);
     CK(d_rec_off.ensure(m)); CK(d_ss.ensure((size_t)cols)); CK(d_L.ensure(m));
     CK(cudaMemcpyAsync(d_rec_off.p, rec_off.data(), (size_t)m * 8, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(d_ss.p, ssb.data(), (size_t)cols, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(d_L.p, Ls.data() + t0, (size_t)m * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(d_L.p, L.data(), (size_t)m * 4, cudaMemcpyHostToDevice, ctx->stream));
     std::vector<float> tau_h;
     if (tau_on_host) {
       std::vector<float> nm((size_t)C.col_total);
@@ -1019,29 +1055,75 @@ static int db_create_a3m_impl(hhg_ctx* ctx, int n, const char* data, const int64
       CK(d_tau.ensure((size_t)cols));
       CK(cudaMemcpyAsync(d_tau.p, tau_h.data(), (size_t)cols * 4, cudaMemcpyHostToDevice, ctx->stream));
     }
-    pieces.emplace_back(new Piece());
-    Piece& P = *pieces.back();
-    P.first = t0; P.n = m; P.ncols = cols;
-    CK(P.cols.alloc((size_t)cols * 7));
-    CK(P.pav.alloc((size_t)m * 20));
-    ColRec* dst = reinterpret_cast<ColRec*>(P.cols.p);
     const int threads = 128;
     k_msa_prepare<<<(unsigned)((cols + threads - 1) / threads), threads, 0, ctx->stream>>>(
         m, C.d_desc.p, d_rec_off.p, C.A, d_ss.p, A, ctx->lg2.p, ctx->diff.p, dst, cols, d_tr_full,
         tau_on_host ? d_tau.p : nullptr);
     k_hhm_pav<<<(unsigned)(((long long)m * 32 + threads - 1) / threads), threads, 0, ctx->stream>>>(
-        m, d_L.p, d_rec_off.p, dst, nullptr, C.nhmm.p, A, P.pav.p, C.pb.p);
+        m, d_L.p, d_rec_off.p, dst, nullptr, C.nhmm.p, A, pav, C.pb.p);
     ctx->launches += 2;
     CK(cudaGetLastError());
-    if (neff_hmm_out) CK(cudaMemcpyAsync(neff_hmm_out + t0, C.nhmm.p, (size_t)m * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    if (neff_out) CK(cudaMemcpyAsync(neff_out, C.nhmm.p, (size_t)m * 4, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));     // host staging of the group is reused by the next one
+    return HHG_OK;
+  }
+};
+
+// The parameter checks of the alignment loaders; `who` prefixes an error.
+static int msa_load_args(const char* who, const hhg_seqdb* sq, const hhg_msa_params* mp, const float* S,
+                         const hhg_prep_params* pp, const float* R, HhmPrepArgs* A) {
+  int rc = msa_params_check(mp);
+  if (rc != HHG_OK) return rc;
+  if ((rc = seqdb_check(sq)) != HHG_OK) return rc;
+  if (mp->qsc > -10.f && !S) return fail(HHG_EINVAL, "%s: the qsc filter needs the substitution matrix S", who);
+  return hhm_prep_args(who, pp, R, A);
+}
+
+static int db_create_a3m_impl(hhg_ctx* ctx, int n, const char* data, const int64_t* off, const int64_t* len,
+                              const hhg_seqdb* sq, const hhg_msa_params* mp, const float* S, const float* pb,
+                              const hhg_prep_params* pp, const float* R, hhg_db** out, float* d_tr_full,
+                              float* neff_hmm_out) {
+  if (!ctx || !out || n <= 0 || !data || !off || !len || !pp || !R || !pb)
+    return fail(HHG_EINVAL, "hhg_db_create_a3m: bad argument");
+  MsaBuilder B;
+  int rc = msa_load_args("hhg_db_create_a3m", sq, mp, S, pp, R, &B.A);
+  if (rc != HHG_OK) return rc;
+  B.ctx = ctx; B.T = RecText{data, off, len}; B.sq = sq; B.mp = mp; B.S = S; B.pb = pb; B.pp = pp;
+  CK(cudaSetDevice(ctx->device));
+  const bool timing = getenv("HHG_TIMING") != nullptr;
+  const auto t_begin = std::chrono::steady_clock::now();
+  double ms_scan = 0.0, ms_kernels = 0.0;
+
+  // The records go through in groups of the builder; each group's column records land in a device piece and the
+  // shard is assembled from the pieces at the end (a database of alignments is far larger than the shard it turns into).
+  struct Piece { DevBuf<float4> cols; DevBuf<float> pav; int first = 0, n = 0; long long ncols = 0; };
+  std::vector<std::unique_ptr<Piece>> pieces;
+  std::vector<int32_t> Ls(n), all(n);
+  std::iota(all.begin(), all.end(), 0);
+  int t0 = 0;
+  while (t0 < n) {
+    const int t1 = B.group_end(all.data(), t0, n, nullptr);
+    const int m = t1 - t0;
+    const auto t_s0 = std::chrono::steady_clock::now();
+    if ((rc = B.scan(all.data() + t0, m)) != HHG_OK) return rc;
+    std::copy(B.L.begin(), B.L.end(), Ls.begin() + t0);
+    ms_scan += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_s0).count();
+    const auto t_c0 = std::chrono::steady_clock::now();
+    pieces.emplace_back(new Piece());
+    Piece& P = *pieces.back();
+    P.first = t0; P.n = m; P.ncols = B.cols;
+    CK(P.cols.alloc((size_t)B.cols * 7));
+    CK(P.pav.alloc((size_t)m * 20));
+    rc = B.build(true, reinterpret_cast<ColRec*>(P.cols.p), P.pav.p, d_tr_full, neff_hmm_out ? neff_hmm_out + t0 : nullptr);
+    if (rc != HHG_OK) return rc;
+    ms_kernels += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_c0).count();
     t0 = t1;
   }
   std::unique_ptr<hhg_db> holder;
   rc = db_new(ctx, n, Ls.data(), true, "record", &holder);
   if (rc != HHG_OK) return rc;
   hhg_db* db = holder.get();
-  db->has_ss = any_ss;
+  db->has_ss = B.any_ss;
   long long at = 0;
   for (auto& pc : pieces) {
     CK(cudaMemcpyAsync(db->cols_raw.p + (size_t)at * 7, pc->cols.p, (size_t)pc->ncols * 7 * sizeof(float4), cudaMemcpyDeviceToDevice, ctx->stream));
@@ -1053,8 +1135,8 @@ static int db_create_a3m_impl(hhg_ctx* ctx, int n, const char* data, const int64
   pieces.clear();
   if (timing) {
     const double ms_all = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
-    fprintf(stderr, "[hhg] alignment loader: %d records, host scan %.1f ms, staging + filter/weights/M-state/finish kernels %.1f ms, "
-                    "rest (pseudocounts, pav, copies) %.1f ms\n", n, ms_scan, ms_kernels, ms_all - ms_scan - ms_kernels);
+    fprintf(stderr, "[hhg] alignment loader: %d records, host scan %.1f ms, kernels %.1f ms, rest (copies) %.1f ms\n",
+            n, ms_scan, ms_kernels, ms_all - ms_scan - ms_kernels);
   }
   return HHG_OK;
 }
@@ -1089,46 +1171,51 @@ int hhg_hhm_parse(const char* rec, int64_t len, int32_t L, int32_t* f_mb, int32_
   return HHG_OK;
 }
 
-static int db_create_hhm_impl(hhg_ctx* ctx, int n, const char* data, const int64_t* off, const int64_t* len,
-                              const hhg_prep_params* pp, const float* R, hhg_db** out, float* d_tr_full) {
-  if (!ctx || !out || n <= 0 || !data || !off || !len || !pp || !R)
-    return fail(HHG_EINVAL, "hhg_db_create_hhm: bad argument");
-  HhmPrepArgs A;
-  int rc = hhm_prep_args("hhg_db_create_hhm", pp, R, &A);
-  if (rc != HHG_OK) return rc;
-  const bool tau_on_host = pp->pcm == 2 && pp->pcc != 1.0f;   // needs the C library's powf: computed per column below
-  CK(cudaSetDevice(ctx->device));
-  // pass 1: lengths (LENG) and whether any record predicts secondary structure
-  std::vector<int32_t> Ls(n);
-  bool any_ss = false;
-  for (int k = 0; k < n; ++k) {
-    int32_t has_ss = 0;
-    HhmScanner sc(data + off[k], len[k]);
-    if (len[k] <= 0 || !sc.peek(&Ls[k], &has_ss)) return fail(HHG_EINVAL, "record %d: no LENG line / not an HHM record", k);
-    any_ss |= has_ss != 0;
-  }
-  std::unique_ptr<hhg_db> holder;
-  if ((rc = db_new(ctx, n, Ls.data(), true, "record", &holder)) != HHG_OK) return rc;
-  hhg_db* db = holder.get();
-  db->has_ss = any_ss;
-
-  // pass 2: chunks of records -> host staging (parsed by a few threads) -> device -> k_hhm_prepare / k_hhm_pav
-  const long long kChunkCols = 2000000;
-  DevBuf<int32_t> d_f, d_trn, d_null, d_haspc;
+// HHM records -> raw column records and pav, one chunk at a time (the shape of MsaBuilder): peek() reads the LENG
+// lines, scan() parses a chunk on the host threads, build() runs k_hhm_prepare and k_hhm_pav and writes the chunk's
+// records to dst and its pav rows to pav.  The HHM shard loader and the stage of a record-sourced shard both use it.
+struct HhmBuilder {
+  hhg_ctx* ctx = nullptr;
+  RecText T{};
+  const hhg_prep_params* pp = nullptr;
+  HhmPrepArgs A{};
+  HhmStaging st;
+  DevBuf<int32_t> d_f, d_trn, d_null, d_haspc, d_L;
   DevBuf<uint8_t> d_ss;
   DevBuf<float> d_neff, d_tau;
   DevBuf<long long> d_coff;
-  std::vector<float> tau_h;
-  HhmStaging st;
-  std::vector<long long> coff;
-  int t0 = 0;
-  while (t0 < n) {
-    int t1 = t0;
-    long long cols = 0;
-    while (t1 < n && (cols == 0 || cols + db->L[t1] <= kChunkCols)) cols += db->L[t1++];
-    const int m = t1 - t0;
-    coff.resize(m);
-    for (int k = 0; k < m; ++k) coff[k] = db->col_off[t0 + k] - db->col_off[t0];
+  std::vector<int32_t> rec, L;         // the scanned chunk: record indices and their lengths
+  std::vector<long long> rec_off;      // first output column of each record of the chunk
+  long long cols = 0;
+  bool any_ss = false;                 // some record peeked so far predicts secondary structure
+
+  // end of the chunk that starts at r[k0] of r[0..n): 2 M columns; Lrec: lengths by record index
+  int group_end(const int32_t* r, int k0, int n, const int32_t* Lrec) const {
+    const long long kChunkCols = 2000000;
+    int k1 = k0;
+    long long c = 0;
+    while (k1 < n && (c == 0 || c + Lrec[r[k1]] <= kChunkCols)) c += Lrec[r[k1++]];
+    return k1;
+  }
+  // LENG of records r[0..m) into Lout[0..m) (not range checked) and whether any predicts secondary structure
+  int peek(const int32_t* r, int m, int32_t* Lout) {
+    for (int k = 0; k < m; ++k) {
+      int32_t has_ss = 0;
+      HhmScanner sc(T.data + T.off[r[k]], T.len[r[k]]);
+      if (T.len[r[k]] <= 0 || !sc.peek(&Lout[k], &has_ss)) return fail(HHG_EINVAL, "record %d: no LENG line / not an HHM record", r[k]);
+      any_ss |= has_ss != 0;
+    }
+    return HHG_OK;
+  }
+
+  int scan(const int32_t* r, int m) {
+    rec.clear();
+    L.resize(m);
+    int rc = peek(r, m, L.data());
+    if (rc != HHG_OK) return rc;
+    rec_off.resize(m);
+    cols = 0;
+    for (int k = 0; k < m; ++k) { rec_off[k] = cols; cols += L[k]; }
     st.f_mb.assign((size_t)cols * 20, 0);
     st.trn_mb.assign((size_t)(cols + m) * 10, 0);
     st.ss.assign((size_t)cols, 0);
@@ -1136,44 +1223,84 @@ static int db_create_hhm_impl(hhg_ctx* ctx, int n, const char* data, const int64
     st.neff_hmm.assign(m, 0.f);
     st.has_pc.assign(m, 0);
     const HostFail bad = host_for(m, [&](int k) {
-      HhmScanner sc(data + off[t0 + k], len[t0 + k]);
-      return sc.parse(db->L[t0 + k], st.f_mb.data() + (size_t)coff[k] * 20,
-                      st.trn_mb.data() + (size_t)(coff[k] + k) * 10, st.ss.data() + coff[k],
+      HhmScanner sc(T.data + T.off[r[k]], T.len[r[k]]);
+      return sc.parse(L[k], st.f_mb.data() + (size_t)rec_off[k] * 20,
+                      st.trn_mb.data() + (size_t)(rec_off[k] + k) * 10, st.ss.data() + rec_off[k],
                       st.null_mb.data() + (size_t)k * 20, &st.neff_hmm[k], &st.has_pc[k]);
     });
-    if (bad.k >= 0) return fail(HHG_EINVAL, "record %d: %s", t0 + bad.k, bad.msg.c_str());
+    if (bad.k >= 0) return fail(HHG_EINVAL, "record %d: %s", r[bad.k], bad.msg.c_str());
+    rec.assign(r, r + m);
+    return HHG_OK;
+  }
+
+  // ss: write the ss bytes of the records (else 0); d_tr_full: hhg_query_from_hhm's linear transitions (one record);
+  // neff_out: Neff_HMM of each record (host)
+  int build(bool ss, ColRec* dst, float* pav, float* d_tr_full, float* neff_out) {
+    const int m = (int)rec.size();
+    const bool tau_on_host = pp->pcm == 2 && pp->pcc != 1.0f;   // needs the C library's powf: computed per column here
     CK(d_f.ensure(st.f_mb.size())); CK(d_trn.ensure(st.trn_mb.size())); CK(d_ss.ensure(st.ss.size()));
-    CK(d_null.ensure(st.null_mb.size())); CK(d_haspc.ensure(m)); CK(d_neff.ensure(m)); CK(d_coff.ensure(m));
+    CK(d_null.ensure(st.null_mb.size())); CK(d_haspc.ensure(m)); CK(d_neff.ensure(m)); CK(d_coff.ensure(m)); CK(d_L.ensure(m));
     CK(cudaMemcpyAsync(d_f.p, st.f_mb.data(), st.f_mb.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(d_trn.p, st.trn_mb.data(), st.trn_mb.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(d_ss.p, st.ss.data(), st.ss.size(), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(d_null.p, st.null_mb.data(), st.null_mb.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(d_haspc.p, st.has_pc.data(), (size_t)m * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(d_neff.p, st.neff_hmm.data(), (size_t)m * 4, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(d_coff.p, coff.data(), (size_t)m * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(d_coff.p, rec_off.data(), (size_t)m * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(d_L.p, L.data(), (size_t)m * 4, cudaMemcpyHostToDevice, ctx->stream));
+    std::vector<float> tau_h;
     if (tau_on_host) {
       tau_h.resize((size_t)cols);
       for (int k = 0; k < m; ++k) {
-        const int32_t* rows = st.trn_mb.data() + (size_t)(coff[k] + k) * 10;
-        for (int j = 1; j <= db->L[t0 + k]; ++j) {
+        const int32_t* rows = st.trn_mb.data() + (size_t)(rec_off[k] + k) * 10;
+        for (int j = 1; j <= L[k]; ++j) {
           const float nM = (float)rows[(size_t)j * 10 + 7] / 1000.0f;
-          tau_h[(size_t)coff[k] + j - 1] = column_tau(pp, nM);
+          tau_h[(size_t)rec_off[k] + j - 1] = column_tau(pp, nM);
         }
       }
       CK(d_tau.ensure((size_t)cols));
       CK(cudaMemcpyAsync(d_tau.p, tau_h.data(), (size_t)cols * 4, cudaMemcpyHostToDevice, ctx->stream));
     }
-    ColRec* dst = reinterpret_cast<ColRec*>(db->cols_raw.p) + db->col_off[t0];
     const int threads = 128;
     k_hhm_prepare<<<(unsigned)((cols + threads - 1) / threads), threads, 0, ctx->stream>>>(
-        m, db->dL.p + t0, d_coff.p, d_f.p, d_trn.p, any_ss ? d_ss.p : nullptr, d_haspc.p, A, ctx->lg2.p,
-        ctx->diff.p, dst, cols, d_tr_full,    // d_tr_full only with a single chunk (hhg_query_from_hhm: one record)
-        tau_on_host ? d_tau.p : nullptr);
+        m, d_L.p, d_coff.p, d_f.p, d_trn.p, ss ? d_ss.p : nullptr, d_haspc.p, A, ctx->lg2.p,
+        ctx->diff.p, dst, cols, d_tr_full, tau_on_host ? d_tau.p : nullptr);
     k_hhm_pav<<<(unsigned)(((long long)m * 32 + threads - 1) / threads), threads, 0, ctx->stream>>>(
-        m, db->dL.p + t0, d_coff.p, dst, d_null.p, d_neff.p, A, db->pav.p + (size_t)t0 * 20);
+        m, d_L.p, d_coff.p, dst, d_null.p, d_neff.p, A, pav);
     ctx->launches += 2;
     CK(cudaGetLastError());
+    if (neff_out) memcpy(neff_out, st.neff_hmm.data(), (size_t)m * 4);
     CK(cudaStreamSynchronize(ctx->stream));   // staging is reused by the next chunk
+    return HHG_OK;
+  }
+};
+
+static int db_create_hhm_impl(hhg_ctx* ctx, int n, const char* data, const int64_t* off, const int64_t* len,
+                              const hhg_prep_params* pp, const float* R, hhg_db** out, float* d_tr_full) {
+  if (!ctx || !out || n <= 0 || !data || !off || !len || !pp || !R)
+    return fail(HHG_EINVAL, "hhg_db_create_hhm: bad argument");
+  HhmBuilder B;
+  int rc = hhm_prep_args("hhg_db_create_hhm", pp, R, &B.A);
+  if (rc != HHG_OK) return rc;
+  B.ctx = ctx; B.T = RecText{data, off, len}; B.pp = pp;
+  CK(cudaSetDevice(ctx->device));
+  // pass 1: lengths (LENG) and whether any record predicts secondary structure
+  std::vector<int32_t> Ls(n), all(n);
+  std::iota(all.begin(), all.end(), 0);
+  if ((rc = B.peek(all.data(), n, Ls.data())) != HHG_OK) return rc;
+  const bool any_ss = B.any_ss;
+  std::unique_ptr<hhg_db> holder;
+  if ((rc = db_new(ctx, n, Ls.data(), true, "record", &holder)) != HHG_OK) return rc;
+  hhg_db* db = holder.get();
+  db->has_ss = any_ss;
+  // pass 2: chunks of records -> host staging (parsed by a few threads) -> device -> k_hhm_prepare / k_hhm_pav
+  int t0 = 0;
+  while (t0 < n) {
+    const int t1 = B.group_end(all.data(), t0, n, Ls.data());
+    if ((rc = B.scan(all.data() + t0, t1 - t0)) != HHG_OK) return rc;
+    // d_tr_full only with a single chunk (hhg_query_from_hhm: one record)
+    rc = B.build(any_ss, reinterpret_cast<ColRec*>(db->cols_raw.p) + db->col_off[t0], db->pav.p + (size_t)t0 * 20, d_tr_full, nullptr);
+    if (rc != HHG_OK) return rc;
     t0 = t1;
   }
   return db_publish_raw(ctx, holder, out);
@@ -1445,6 +1572,7 @@ int hhg_db_destroy(hhg_db* db) {
   if (db) {
     cudaSetDevice(db->device);
     if (db->store) db->store->users--;
+    if (db->src) db->src->users--;
     delete db;
   }
   return HHG_OK;
@@ -1557,16 +1685,14 @@ int hhg_dbstore_append_db(hhg_ctx* ctx, hhg_dbstore* store, const hhg_db* db) {
   return HHG_OK;
 }
 
-int hhg_db_create_staged(hhg_ctx* ctx, hhg_dbstore* store, int max_targets, long long max_cols, hhg_db** out) {
-  if (!ctx || !store || !out || max_targets < 1 || max_cols < 1) return fail(HHG_EINVAL, "hhg_db_create_staged: bad argument");
-  if (store->device != ctx->device)
-    return fail(HHG_EINVAL, "hhg_db_create_staged: the store is mapped for device %d, ctx is on %d", store->device, ctx->device);
+// An empty staged shard of max_targets slots over an arena of max_cols records.
+static int staged_new(hhg_ctx* ctx, int max_targets, long long max_cols, bool has_ss, std::unique_ptr<hhg_db>* out) {
   CK(cudaSetDevice(ctx->device));
   std::unique_ptr<hhg_db> db(new hhg_db());
   db->device = ctx->device;
   db->n = max_targets;
   db->total_cols = max_cols;
-  db->has_ss = store->has_ss;
+  db->has_ss = has_ss;
   db->L.assign(max_targets, 0);
   db->col_off.assign(max_targets, 0);
   db->raw = true;
@@ -1589,6 +1715,17 @@ int hhg_db_create_staged(hhg_ctx* ctx, hhg_dbstore* store, int max_targets, long
   CK(cudaMemsetAsync(db->cols.p, 0, (size_t)max_cols * sizeof(ColRec), ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   db->stage.reset(new StageCache(max_targets, max_cols));
+  *out = std::move(db);
+  return HHG_OK;
+}
+
+int hhg_db_create_staged(hhg_ctx* ctx, hhg_dbstore* store, int max_targets, long long max_cols, hhg_db** out) {
+  if (!ctx || !store || !out || max_targets < 1 || max_cols < 1) return fail(HHG_EINVAL, "hhg_db_create_staged: bad argument");
+  if (store->device != ctx->device)
+    return fail(HHG_EINVAL, "hhg_db_create_staged: the store is mapped for device %d, ctx is on %d", store->device, ctx->device);
+  std::unique_ptr<hhg_db> db;
+  int rc = staged_new(ctx, max_targets, max_cols, store->has_ss, &db);
+  if (rc != HHG_OK) return rc;
   db->store = store;
   store->users++;
   *out = db.release();
@@ -1603,11 +1740,19 @@ static int stage_ctas() {
   return x > 0 ? x : 32;
 }
 
+template <class B>
+static int stage_records(hhg_ctx* ctx, hhg_db* db, B& b, int n, const int32_t* ids, int32_t* local_out,
+                         hhg_stage_stats* stats_out);
+
 int hhg_db_stage(hhg_ctx* ctx, hhg_db* db, int n, const int32_t* global_ids, int32_t* local_ids_out,
                  hhg_stage_stats* stats_out) {
   if (!ctx || !db || n < 0 || (n && (!global_ids || !local_ids_out))) return fail(HHG_EINVAL, "hhg_db_stage: bad argument");
   if (!db->stage) return fail(HHG_EINVAL, "hhg_db_stage: the shard was not made by hhg_db_create_staged");
   if (db->device != ctx->device) return fail(HHG_EINVAL, "db lives on device %d, ctx on %d", db->device, ctx->device);
+  if (db->src) {
+    if (db->src->kind == 0) return stage_records(ctx, db, *std::static_pointer_cast<HhmBuilder>(db->builder), n, global_ids, local_ids_out, stats_out);
+    return stage_records(ctx, db, *std::static_pointer_cast<MsaBuilder>(db->builder), n, global_ids, local_ids_out, stats_out);
+  }
   const hhg_dbstore* st = db->store;
   std::vector<StageItem> items;
   std::vector<int> freed;
@@ -1668,6 +1813,239 @@ int hhg_db_staged_lookup(const hhg_db* db, int n, const int32_t* local_ids, int3
     if (s < 0 || s >= db->n) return fail(HHG_EINVAL, "hhg_db_staged_lookup: local id %d out of range", s);
     if (global_ids_out) global_ids_out[k] = db->stage->global_of(s);
     if (first_col_out) first_col_out[k] = db->stage->off_of(s);
+  }
+  return HHG_OK;
+}
+
+// ------------------------------------------------------------------------- record source + staged shard over it
+// What prefilter_db + HHEntry::getTemplateHMM do (src/hhprefilter.cpp:561-590, src/hhdatabase.cpp:300-336,
+// :398-461): only the survivors' records are ever parsed, when hhg_db_stage makes them resident (DESIGN 4.12).
+static int recsrc_new(hhg_ctx* ctx, const char* who, int kind, int n, const char* data, const int64_t* off,
+                      const int64_t* len, const hhg_seqdb* seqs, const hhg_msa_params* mp, const float* S,
+                      const float* pb, const hhg_prep_params* pp, const float* R, int has_ss, hhg_recsrc** out) {
+  if (!ctx || !out || n < 1 || !data || !off || !len || !pp || !R || (kind && !pb))
+    return fail(HHG_EINVAL, "%s: bad argument", who);
+  HhmPrepArgs A;
+  int rc = kind ? msa_load_args(who, seqs, mp, S, pp, R, &A) : hhm_prep_args(who, pp, R, &A);
+  if (rc != HHG_OK) return rc;
+  for (int k = 0; k < n; ++k)
+    if (off[k] < 0 || len[k] < 0) return fail(HHG_EINVAL, "%s: record %d: offset %lld, length %lld", who, k, (long long)off[k], (long long)len[k]);
+  std::unique_ptr<hhg_recsrc> src(new hhg_recsrc());
+  src->device = ctx->device;
+  src->kind = kind;
+  src->n = n;
+  src->data = data;
+  src->off.assign(off, off + n);
+  src->len.assign(len, len + n);
+  if (seqs) src->seqs = *seqs;
+  if (mp) src->mp = *mp;
+  src->pp = *pp;
+  if (S) src->S.assign(S, S + 400);
+  if (pb) src->pb.assign(pb, pb + 20);
+  src->R.assign(R, R + 400);
+  src->has_ss = has_ss != 0;
+  src->L.assign(n, 0);
+  *out = src.release();
+  return HHG_OK;
+}
+
+int hhg_recsrc_create_hhm(hhg_ctx* ctx, int n, const char* data, const int64_t* off, const int64_t* len,
+                          const hhg_prep_params* pp, const float* R, int has_ss, hhg_recsrc** out) {
+  return recsrc_new(ctx, "hhg_recsrc_create_hhm", 0, n, data, off, len, nullptr, nullptr, nullptr, nullptr, pp, R, has_ss, out);
+}
+
+int hhg_recsrc_create_a3m(hhg_ctx* ctx, int n, const char* data, const int64_t* off, const int64_t* len,
+                          const hhg_msa_params* mp, const float* S, const float* pb, const hhg_prep_params* pp,
+                          const float* R, int has_ss, hhg_recsrc** out) {
+  return recsrc_new(ctx, "hhg_recsrc_create_a3m", 1, n, data, off, len, nullptr, mp, S, pb, pp, R, has_ss, out);
+}
+
+int hhg_recsrc_create_ca3m(hhg_ctx* ctx, int n, const char* data, const int64_t* off, const int64_t* len,
+                           const hhg_seqdb* seqs, const hhg_msa_params* mp, const float* S, const float* pb,
+                           const hhg_prep_params* pp, const float* R, int has_ss, hhg_recsrc** out) {
+  if (!seqs) return fail(HHG_EINVAL, "hhg_recsrc_create_ca3m: the sequence database is NULL");
+  return recsrc_new(ctx, "hhg_recsrc_create_ca3m", 2, n, data, off, len, seqs, mp, S, pb, pp, R, has_ss, out);
+}
+
+int hhg_recsrc_destroy(hhg_recsrc* src) {
+  if (!src) return HHG_OK;
+  if (src->users > 0) return fail(HHG_EINVAL, "hhg_recsrc_destroy: %d staged shards still use the record source", src->users);
+  delete src;
+  return HHG_OK;
+}
+
+int hhg_recsrc_size(const hhg_recsrc* src) { return src ? src->n : 0; }
+
+int hhg_db_create_staged_records(hhg_ctx* ctx, hhg_recsrc* src, int max_targets, long long max_cols, hhg_db** out) {
+  if (!ctx || !src || !out || max_targets < 1 || max_cols < 1) return fail(HHG_EINVAL, "hhg_db_create_staged_records: bad argument");
+  if (src->device != ctx->device)
+    return fail(HHG_EINVAL, "hhg_db_create_staged_records: the record source was made for device %d, ctx is on %d", src->device, ctx->device);
+  std::unique_ptr<hhg_db> db;
+  int rc = staged_new(ctx, max_targets, max_cols, src->has_ss, &db);
+  if (rc != HHG_OK) return rc;
+  const RecText T{src->data, src->off.data(), src->len.data()};
+  if (src->kind == 0) {
+    auto b = std::make_shared<HhmBuilder>();
+    b->T = T; b->pp = &src->pp;
+    if ((rc = hhm_prep_args("hhg_db_create_staged_records", &src->pp, src->R.data(), &b->A)) != HHG_OK) return rc;
+    db->builder = b;
+  } else {
+    auto b = std::make_shared<MsaBuilder>();
+    b->T = T; b->sq = src->kind == 2 ? &src->seqs : nullptr; b->mp = &src->mp;
+    b->S = src->S.empty() ? nullptr : src->S.data(); b->pb = src->pb.data(); b->pp = &src->pp;
+    if ((rc = hhm_prep_args("hhg_db_create_staged_records", &src->pp, src->R.data(), &b->A)) != HHG_OK) return rc;
+    db->builder = b;
+  }
+  db->neff.assign(max_targets, 0.f);
+  db->src = src;
+  src->users++;
+  *out = db.release();
+  return HHG_OK;
+}
+
+// The error just recorded, prefixed with the entry point's name.
+static int stage_error(int rc) {
+  const std::string msg = hhg_last_error();
+  return fail(rc, "hhg_db_stage: %s", msg.c_str());
+}
+
+// After a failure between the placement and the last gather the slot tables no longer describe the arena: every
+// slot is emptied (a new identity, as for any call that changes a slot).
+static void stage_clear(hhg_ctx* ctx, hhg_db* db) {
+  db->stage.reset(new StageCache(db->n, db->total_cols));
+  std::fill(db->L.begin(), db->L.end(), 0);
+  std::fill(db->col_off.begin(), db->col_off.end(), 0);
+  std::fill(db->neff.begin(), db->neff.end(), 0.f);
+  cudaMemsetAsync(db->dL.p, 0, (size_t)db->n * 4, ctx->stream);
+  cudaStreamSynchronize(ctx->stream);
+  db->serial = g_db_serial.fetch_add(1);
+  db->cols_version++;
+  db->prepared = false;
+}
+
+// hhg_db_stage on a record-sourced shard: the request's missing records are scanned on the host threads (their lengths
+// and every parse error before anything changes), StageCache places them exactly as it places a store's targets, and
+// the targets to copy are built in groups by the loaders' builder into rec_cols / rec_pav, from where k_stage_gather
+// moves them into their arena runs.  A re-layout of the request's own residents rebuilds them from their records.
+// The host is blocked for the scan and the build.
+template <class B>
+static int stage_records(hhg_ctx* ctx, hhg_db* db, B& b, int n, const int32_t* ids, int32_t* local_out,
+                         hhg_stage_stats* stats_out) {
+  hhg_recsrc* src = db->src;
+  CK(cudaSetDevice(ctx->device));
+  b.ctx = ctx;
+  const bool timing = getenv("HHG_TIMING") != nullptr;
+  const auto t_begin = std::chrono::steady_clock::now();
+  // 1. the distinct missing records, in the order StageCache will place them
+  std::vector<int32_t> miss;
+  {
+    std::unordered_set<int> seen;
+    for (int k = 0; k < n; ++k) {
+      const int g = ids[k];
+      if (g < 0 || g >= src->n)
+        return fail(HHG_EINVAL, "hhg_db_stage: request %d: target id %d outside the record source (%d records)", k, g, src->n);
+      if (db->stage->slot_of(g) < 0 && seen.insert(g).second) miss.push_back(g);
+    }
+  }
+  // 2-3. their lengths: LENG lines of HHM records (peek), then the full parse of every group, which also refuses a
+  // malformed alignment; the parse of the last group stays in b and is used again below when it is what gets built
+  const int nm = (int)miss.size();
+  std::vector<int32_t> Lm(nm);
+  int rc = b.peek(miss.data(), nm, Lm.data());
+  if (rc != HHG_OK) return stage_error(rc);
+  if (std::is_same<B, HhmBuilder>::value) {
+    for (int k = 0; k < nm; ++k)
+      if (Lm[k] < 1 || Lm[k] > 32767) return fail(HHG_EINVAL, "hhg_db_stage: record %d: length %d out of [1,32767]", miss[k], Lm[k]);
+    for (int k = 0; k < nm; ++k) src->L[miss[k]] = Lm[k];
+  }
+  for (int k0 = 0, k1; k0 < nm; k0 = k1) {
+    k1 = b.group_end(miss.data(), k0, nm, src->L.data());
+    if ((rc = b.scan(miss.data() + k0, k1 - k0)) != HHG_OK) return stage_error(rc);
+    for (int k = 0; k < k1 - k0; ++k) src->L[b.rec[k]] = b.L[k];
+  }
+  const double ms_scan = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+  // 4. placement (the record offsets stand in for store offsets: every item's source is replaced below)
+  static_assert(sizeof(int64_t) == sizeof(long long), "record offsets as StageCache source offsets");
+  std::vector<StageItem> items;
+  std::vector<int> freed;
+  StageStats ss{};
+  int bad = 0;
+  long long need_slots = 0, need_cols = 0;
+  rc = db->stage->request(n, ids, src->n, src->L.data(), reinterpret_cast<const long long*>(src->off.data()), local_out,
+                          &items, &freed, &ss, &bad, &need_slots, &need_cols);
+  if (rc == -1) return fail(HHG_EINVAL, "hhg_db_stage: request %d: target id %d outside the record source (%d records)", bad, ids[bad], src->n);
+  if (rc == -2)
+    return fail(HHG_EINVAL, "hhg_db_stage: the request needs %lld slots and %lld columns, the staged shard has %d and %lld",
+                need_slots, need_cols, db->n, db->total_cols);
+  if (stats_out) memcpy(stats_out, &ss, sizeof ss);
+  if (items.empty() && freed.empty()) return HHG_OK;
+  for (const StageItem& it : items) { db->L[it.slot] = it.len; db->col_off[it.slot] = it.dst; }
+  for (int s : freed) db->L[s] = 0;
+  db->serial = g_db_serial.fetch_add(1);
+  db->cols_version++;
+  db->prepared = false;
+  // 5-6. build the copied targets group by group, each group gathered from the scratch into its arena runs; descriptor
+  // k of a group reads scratch records from the builder's rec_off[k] and pav row k
+  const int ni = (int)items.size();
+  std::vector<int32_t> order(ni);
+  for (int k = 0; k < ni; ++k) order[k] = items[k].global;
+  std::vector<StageDesc> desc;
+  std::vector<float> neff;
+  double ms_build = 0.0, ms_gather = 0.0;
+  for (int k0 = 0, k1; k0 < ni; k0 = k1) {
+    const auto t0 = std::chrono::steady_clock::now();
+    k1 = b.group_end(order.data(), k0, ni, src->L.data());
+    const int m = k1 - k0;
+    if (!((int)b.rec.size() == m && std::equal(b.rec.begin(), b.rec.end(), order.begin() + k0)) &&
+        (rc = b.scan(order.data() + k0, m)) != HHG_OK) {
+      stage_clear(ctx, db);
+      return stage_error(rc);
+    }
+    neff.resize(m);
+    cudaError_t e = db->rec_cols.ensure((size_t)b.cols * 7);
+    if (e == cudaSuccess) e = db->rec_pav.ensure((size_t)m * 20);
+    rc = e == cudaSuccess ? b.build(src->has_ss, reinterpret_cast<ColRec*>(db->rec_cols.p), db->rec_pav.p, nullptr, neff.data())
+                          : fail(HHG_ECUDA, "%s", cudaGetErrorString(e));
+    if (rc != HHG_OK) { stage_clear(ctx, db); return stage_error(rc); }
+    const auto t1 = std::chrono::steady_clock::now();
+    ms_build += std::chrono::duration<double, std::milli>(t1 - t0).count();
+    desc.clear();
+    long long runs = 0;
+    for (int k = 0; k < m; ++k) {
+      const StageItem& it = items[k0 + k];
+      desc.push_back(StageDesc{b.rec_off[k], it.dst, it.len, it.slot, k, (int)runs});
+      runs += (it.len + kStageRun - 1) / kStageRun;
+      db->neff[it.slot] = neff[k];
+    }
+    if (k0 == 0)
+      for (int s : freed) desc.push_back(StageDesc{0, 0, 0, s, 0, (int)runs});
+    e = db->d_desc.ensure(desc.size());
+    if (e == cudaSuccess) e = cudaMemcpyAsync(db->d_desc.p, desc.data(), desc.size() * sizeof(StageDesc), cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) {
+      const int ctas = (int)std::max(1LL, std::min<long long>(stage_ctas(), std::max<long long>((runs + 7) / 8, ((long long)desc.size() + 31) / 32)));
+      k_stage_gather<<<ctas, 256, 0, ctx->stream>>>((int)desc.size(), (int)runs, db->d_desc.p, db->rec_cols.p, db->rec_pav.p,
+                                                    db->cols_raw.p, db->pav.p, db->dL.p, db->dcol_off.p);
+      ctx->launches++;
+      e = cudaGetLastError();
+    }
+    if (e == cudaSuccess && timing) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { stage_clear(ctx, db); return fail(HHG_ECUDA, "hhg_db_stage: %s", cudaGetErrorString(e)); }
+    ms_gather += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count();
+  }
+  if (timing)
+    fprintf(stderr, "[hhg] record stage: %d missing records, %d built, host scan %.3f ms, build %.3f ms, gather %.3f ms\n",
+            nm, ni, ms_scan, ms_build, ms_gather);
+  return HHG_OK;
+}
+
+int hhg_db_staged_neff(const hhg_db* db, int n, const int32_t* local_ids, float* neff_out) {
+  if (!db || !db->stage || n < 0 || (n && (!local_ids || !neff_out))) return fail(HHG_EINVAL, "hhg_db_staged_neff: bad argument / shard not staged");
+  if (!db->src) return fail(HHG_EINVAL, "hhg_db_staged_neff: the shard stages from a store of packed records, which holds no Neff");
+  for (int k = 0; k < n; ++k) {
+    const int s = local_ids[k];
+    if (s < 0 || s >= db->n) return fail(HHG_EINVAL, "hhg_db_staged_neff: local id %d out of range", s);
+    if (db->L[s] < 1) return fail(HHG_EINVAL, "hhg_db_staged_neff: slot %d of the staged shard is empty", s);
+    neff_out[k] = db->neff[s];
   }
   return HHG_OK;
 }

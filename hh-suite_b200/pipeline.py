@@ -52,8 +52,9 @@ def search_batch(ctx: capi.Context, db: capi.TargetDB, csdb: capi.CsDB, queries,
 
 def search_staged(ctx: capi.Context, db: capi.StagedDB, csdb: capi.CsDB, q_p, q_tr, q_pav, lib219, q_prefilter_p=None,
                   altali=4, smin=20.0, cs_names=None, db_names=None, columnscore=1, pb=None, **pf_kwargs):
-    """search() over a database whose profiles stay in host memory (db.store): the prefilter's survivors are staged
-    into db (one hhg_db_stage call), the query's null model is applied to the staged records (columnscore / pb as in
+    """search() over a database whose profiles stay in host memory (db.store: a HostStore, or a RecordSource whose
+    survivors are built from their records as they are staged): the prefilter's survivors are staged into db (one
+    hhg_db_stage call), the query's null model is applied to the staged records (columnscore / pb as in
     TargetDB.apply_null_model) and the same runner aligns them.  Returns what search() returns over a resident raw shard
     of the whole database after apply_null_model(q_pav, pb, columnscore): survivor ids and Hit.target are GLOBAL ids.
     The survivors of one query must fit db (HhgError otherwise, with the sizes needed)."""
@@ -63,6 +64,7 @@ def search_staged(ctx: capi.Context, db: capi.StagedDB, csdb: capi.CsDB, q_p, q_
     if not len(ids):
         return ids, []
     local = db.stage(ids)
+    _check_staged(db, csdb, ids, local, cs_names, db_names)
     db.apply_null_model(q_pav, pb, columnscore)
     ctx.set_query(q_p, q_tr)
     hits = runner.ViterbiRunner(ctx, db, altali=altali, smin=smin).alignment(local)
@@ -85,6 +87,7 @@ def search_batch_staged(ctx: capi.Context, db: capi.StagedDB, csdb: capi.CsDB, q
     if not len(rq):
         return [(x, []) for x in ids]
     local = db.stage(np.concatenate(ids))
+    _check_staged(db, csdb, np.concatenate(ids), local, cs_names, db_names)
     capi.query_set_batch(ctx, [(q[0], q[1]) for q in queries], q_pav=np.stack([q[2] for q in queries]))
     hits = runner.BatchViterbiRunner(ctx, db, altali=altali, smin=smin, columnscore=columnscore, pb=pb).alignment(rq, local)
     return [(x, to_global_hits(db, h)) for x, h in zip(ids, hits)]
@@ -109,10 +112,21 @@ def _to_targets(ids, db, csdb, cs_names, db_names):
         if missing:
             raise KeyError(f"{len(missing)} prefilter hits have no entry in the profile shard, e.g. {missing[0]!r}")
         return np.array([where[cs_names[k]] for k in ids], np.int32)
-    if csdb.n != db.n or not np.array_equal(np.asarray(csdb.Lh), np.asarray(db.Lh)):
-        raise ValueError("cs219 shard and profile shard are not index-aligned (different sizes or lengths): "
-                         "pass cs_names / db_names so the survivors are mapped by name like the reference does")
+    # a record source knows the lengths only of what it has scanned: the count here, each survivor's length once staged
+    if csdb.n != db.n or (not isinstance(db, capi.RecordSource) and not np.array_equal(np.asarray(csdb.Lh), np.asarray(db.Lh))):
+        raise ValueError(_NOT_ALIGNED)
     return ids
+
+
+_NOT_ALIGNED = ("cs219 shard and profile shard are not index-aligned (different sizes or lengths): "
+                "pass cs_names / db_names so the survivors are mapped by name like the reference does")
+
+
+def _check_staged(db: capi.StagedDB, csdb, ids, local, cs_names, db_names):
+    """The length check of _to_targets for survivors staged from a record source: staged length == cs219 length."""
+    if cs_names is None and db_names is None and isinstance(db.store, capi.RecordSource) and \
+            not np.array_equal(np.asarray(db.Lh)[local], np.asarray(csdb.Lh)[ids]):
+        raise ValueError(_NOT_ALIGNED)
 
 
 def translate_cs219(p_cols: np.ndarray, pav_like: np.ndarray, lib219: np.ndarray) -> np.ndarray:

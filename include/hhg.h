@@ -339,6 +339,39 @@ int hhg_db_stage(hhg_ctx* ctx, hhg_db* db, int n, const int32_t* global_ids, int
 int hhg_db_staged_lookup(const hhg_db* db, int n, const int32_t* local_ids, int32_t* global_ids_out,
                          int64_t* first_col_out);
 
+/* A staged shard whose source is the database's own ffindex records (HHM, A3M or compressed A3M) instead of a store:
+ * nothing is parsed or held for a record until a stage call names it, so a database of tens of millions of alignments
+ * needs no store and no load pass.
+ * hhg_recsrc_create_hhm / _a3m / _ca3m: n records, record r = len[r] bytes at data + off[r].  The parameters mean what
+ *   they mean for hhg_db_create_hhm / _a3m / _ca3m and are copied, as are off and len; data and the hhg_seqdb arrays
+ *   are NOT copied or read here: the caller keeps them alive (typically an mmap of the ffdata) while the source lives.
+ *   Creation cost does not depend on the records' size.  GLOBAL ids are record indices.  has_ss = 1 writes the ss
+ *   bytes the resident loaders write (0 for a record without ss_pred); has_ss = 0 writes 0 everywhere, and the shard
+ *   refuses ss searches like a resident shard without ss.
+ * hhg_recsrc_destroy is refused while a staged shard made over the source lives.
+ * hhg_db_create_staged_records: as hhg_db_create_staged over the source.  hhg_db_stage on it places targets exactly as
+ *   over a store (same local ids, stats and evictions for the same id sequence), but the host first scans the request's
+ *   missing records on its threads; a malformed record, a length outside [1, 32767] or an id outside the source is
+ *   HHG_EINVAL naming the record, with the shard unchanged and nothing launched.  The targets to copy are then built in
+ *   groups by the loaders' kernels and moved into their arena runs by k_stage_gather on the context stream.  The call
+ *   blocks the host for the scan and the build.  A record that fails in the kernels (e.g. no sequence left after the
+ *   filter) is HHG_EINVAL naming it and leaves the shard empty.
+ * hhg_db_staged_neff: Neff_HMM of the targets in n slots of a record-sourced shard (hhg_hitlist_pvalues' t_neff);
+ *   refused on a store-backed shard and on an empty slot. */
+typedef struct hhg_recsrc hhg_recsrc;
+int hhg_recsrc_create_hhm(hhg_ctx* ctx, int n, const char* data, const int64_t* off, const int64_t* len,
+                          const hhg_prep_params* pp, const float* R, int has_ss, hhg_recsrc** out);
+int hhg_recsrc_create_a3m(hhg_ctx* ctx, int n, const char* data, const int64_t* off, const int64_t* len,
+                          const hhg_msa_params* mp, const float* S, const float* pb, const hhg_prep_params* pp,
+                          const float* R, int has_ss, hhg_recsrc** out);
+int hhg_recsrc_create_ca3m(hhg_ctx* ctx, int n, const char* data, const int64_t* off, const int64_t* len,
+                           const hhg_seqdb* seqs, const hhg_msa_params* mp, const float* S, const float* pb,
+                           const hhg_prep_params* pp, const float* R, int has_ss, hhg_recsrc** out);
+int hhg_recsrc_destroy(hhg_recsrc* src);
+int hhg_recsrc_size(const hhg_recsrc* src);
+int hhg_db_create_staged_records(hhg_ctx* ctx, hhg_recsrc* src, int max_targets, long long max_cols, hhg_db** out);
+int hhg_db_staged_neff(const hhg_db* db, int n, const int32_t* local_ids, float* neff_out);
+
 /* Set the query (replaces HMMSimd::MapOneHMM).  S33: float[44*44] or NULL (needed iff use_ss). */
 int hhg_query_set(hhg_ctx* ctx, int Lq, const float* p, const float* tr, const uint8_t* ss,
                   const float* S33, const hhg_params* par);
