@@ -68,8 +68,14 @@ class HhmScanner {
       const size_t n = (size_t)(e - p);
       if (n >= 2 && p[0] == '/' && p[1] == '/') break;
       if (blank(p, e) || (n >= 2 && !memcmp(p, "HH", 2))) { p = next; continue; }
-      if (n >= 4 && !memcmp(p, "NEFF", 4)) {
-        *neff_hmm = n > 6 ? strtof(std::string(p + 6, e).c_str(), nullptr) : 0.f;   // sscanf(line+6, "%f")
+      if ((n >= 4 && !memcmp(p, "NEFF", 4)) || (n >= 3 && !memcmp(p, "NAA", 3))) {
+        // sscanf(line+6, "%f", &Neff_HMM) (:296): a line without a number there leaves the value as it was
+        if (n > 6) {
+          const std::string s(p + 6, e);
+          char* stop = nullptr;
+          const float v = strtof(s.c_str(), &stop);
+          if (stop != s.c_str()) *neff_hmm = v;
+        }
       } else if (n >= 3 && !memcmp(p, "PCT", 3)) {
         *has_pc = 1;
       } else if (n >= 4 && !memcmp(p, "NULL", 4)) {
@@ -133,7 +139,10 @@ class HhmScanner {
     }
     if (!have_hmm) return "no HMM section";
     if (!have_null) return "no NULL line";
-    for (int j = 1; j <= L; ++j) ss[j - 1] = (uint8_t)(pred[j] * 11 + conf[j]);   // MAXCF = 11, src/hhhmmsimd.cpp:133
+    // Neff_HMM = 0 would make pav = pb*100/0 = inf and then NaN (CalculateAminoAcidBackground): refuse the record
+    if (*neff_hmm == 0.f) return "Neff_HMM is 0 (no NEFF/NAA line, or NEFF 0)";
+    // a record without ss_pred has no secondary structure, whatever its ss_conf says; ss_pred without ss_conf: conf 0
+    for (int j = 1; j <= L; ++j) ss[j - 1] = pred_seq < 0 ? 0 : (uint8_t)(pred[j] * 11 + conf[j]);   // MAXCF = 11
     return "";
   }
 

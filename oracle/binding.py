@@ -369,7 +369,8 @@ class RefShim:
         if L < 0:
             raise IOError(path)
         return dict(L=L, p=p[:L + 2].copy(), tr=tr[:L + 1].copy(), pav=pav,
-                    ss=(sp[:L + 2] * 11 + sc[:L + 2]).astype(np.uint8), neff=neff.value)
+                    ss=(sp[:L + 2] * 11 + sc[:L + 2]).astype(np.uint8), ss_pred=sp[:L + 2].copy(),
+                    ss_conf=sc[:L + 2].copy(), neff=neff.value)
 
     def prepare_template_hhm_raw(self, path, columnscore=1, maxL=4000):
         p_raw = np.zeros((maxL + 2, 20), np.float32); p_prep = np.zeros((maxL + 2, 20), np.float32)
@@ -379,6 +380,47 @@ class RefShim:
         if L < 0:
             raise IOError(path)
         return dict(L=L, p_raw=p_raw[:L + 2].copy(), p=p_prep[:L + 2].copy(), tr=tr[:L + 1].copy(), pav=pav)
+
+    # Entry points added to the shim after the first shipped builds are bound when first used, so a shim built by an
+    # older recipe still loads; provides() tells whether a build has them.
+    HHM_FAMILY_ENTRY_POINTS = ("hhref_read_hhm_header", "hhref_set_gap", "hhref_set_pb", "hhref_write_hhm")
+
+    def provides(self, *names):
+        return all(hasattr(self.lib, n) for n in names)
+
+    def read_hhm_header(self, path):
+        """HMM::Read of a template file alone -> (L, Neff_HMM, has_pseudocounts); the global pb is left as it was."""
+        fn = self.lib.hhref_read_hhm_header
+        fn.argtypes = [C.c_char_p, C.POINTER(C.c_float), C.POINTER(C.c_int)]
+        neff = C.c_float(); has_pc = C.c_int()
+        L = fn(path.encode(), C.byref(neff), C.byref(has_pc))
+        if L < 0:
+            raise IOError(path)
+        return L, neff.value, has_pc.value
+
+    def set_gap(self, gapb=1.0, gapd=0.15, gape=1.0, gapf=0.6, gapg=0.6, gaph=0.6, gapi=0.6):
+        """par.gapb .. gapi (-gapb .. -gapi) for the following preparations; the arguments' defaults are the
+        reference's (src/hhdecl.cpp), gapb = 0 is hhmake's setting (no transition pseudocounts)."""
+        self.lib.hhref_set_gap.argtypes = [C.c_float] * 7
+        self.lib.hhref_set_gap(gapb, gapd, gape, gapf, gapg, gaph, gapi)
+
+    def set_pb(self, pb):
+        """Put back the global background pb (internal order) that HMM::Read overwrites with each file's NULL line."""
+        pb = np.ascontiguousarray(pb, np.float32)
+        assert pb.shape == (20,)
+        self.lib.hhref_set_pb.argtypes = [c_f32p]
+        self.lib.hhref_set_pb(_p(pb, c_f32p))
+
+    def write_hhm(self, a3m_path, add_pc=False, cap=1 << 24):
+        """hhmake on an A3M file: the HHM text HMM::WriteToFile writes (add_pc: with nocontxt pseudocounts, a PCT record)."""
+        fn = self.lib.hhref_write_hhm
+        fn.restype = C.c_long
+        fn.argtypes = [C.c_char_p, C.c_int, C.c_char_p, C.c_long]
+        buf = C.create_string_buffer(cap)
+        n = fn(a3m_path.encode(), 1 if add_pc else 0, buf, cap)
+        if n < 0:
+            raise IOError(f"hhref_write_hhm({a3m_path}) = {n}")
+        return buf.raw[:n]
 
     def crf_text(self):
         """The context_data.crf bytes embedded in the reference build (what InitializePseudocountsEngine reads)."""

@@ -24,6 +24,7 @@
 #include <float.h>
 #include <math.h>
 #include <stdint.h>
+#include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -440,7 +441,16 @@ int hho_hhm_parse(const char* text, long len, int maxL, float* neff_hmm, int* ha
     if (blank_line(line, end)) continue;
     if (!strncmp(line, "HH", 2)) continue;
     if (!strncmp(line, "LENG", 4)) { const char* q = line + 4; Lstated = next_int(&q, 0, 0); }
-    else if (!strncmp(line, "NEFF", 4)) { *neff_hmm = strtof(line + 6, NULL); }
+    else if (!strncmp(line, "NEFF", 4) || !strncmp(line, "NAA", 3)) {   /* sscanf(line+6, "%f", &Neff_HMM), :296 */
+      const char* e = line;
+      while (e < end && *e != '\n') e++;
+      if (e - line > 6) {
+        char buf[256];
+        size_t n = (size_t)(e - line - 6) < sizeof buf - 1 ? (size_t)(e - line - 6) : sizeof buf - 1;
+        memcpy(buf, line + 6, n); buf[n] = 0;
+        (void)sscanf(buf, "%f", neff_hmm);            /* no number: the value stays */
+      }
+    }
     else if (!strncmp(line, "PCT", 3)) *has_pc = 1;
     else if (!strncmp(line, "SEQ", 3)) {
       int k = -1, l = 1, m = 1;

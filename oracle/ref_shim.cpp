@@ -188,6 +188,45 @@ extern "C" void hhref_set_pc(int mode, float a, float b, float c) {
   g->par->pc_hhm_nocontext_c = c;
 }
 
+// override par.gapb .. gapi (-gapb .. -gapi) for the following preparations; gapb = 0 is hhmake's setting
+extern "C" void hhref_set_gap(float gapb, float gapd, float gape, float gapf, float gapg, float gaph, float gapi) {
+  Parameters& par = *g->par;
+  par.gapb = gapb; par.gapd = gapd; par.gape = gape; par.gapf = gapf; par.gapg = gapg; par.gaph = gaph; par.gapi = gapi;
+}
+
+// HMM::Read overwrites the global background pb with each file's NULL line; this puts a saved one back
+extern "C" void hhref_set_pb(const float* pb20) { memcpy(g->pb, pb20, 20 * sizeof(float)); }
+
+// hhmake's chain for an A3M file (src/hhmake.cpp:389-391): ReadQueryFile (Read, Compress, Shrink, FilterForDisplay,
+// Filter, FrequenciesAndTransitions), PrepareQueryHMM, HMM::WriteToFile.  add_pc = 0: hhmake's defaults gapb = 0 and
+// pcm = 0 (raw frequencies, no PCT line); add_pc = 1: the current gap and nocontxt pseudocount settings (a PCT record).
+// Writes at most cap bytes to out; returns the length of the record text, or < 0.
+extern "C" long hhref_write_hhm(const char* path, int add_pc, char* out, long cap) {
+  Parameters& par = *g->par;
+  const float gapb = par.gapb;
+  const int pcm = par.pc_hhm_nocontext_mode;
+  if (!add_pc) { par.gapb = 0.f; par.pc_hhm_nocontext_mode = 0; }
+  HMM* q = new HMM(MAXSEQDIS, g->maxres);
+  Alignment* ali = new Alignment(par.maxseq, g->maxres);
+  char infile[NAMELEN];
+  strncpy(infile, path, NAMELEN - 1); infile[NAMELEN - 1] = 0;
+  char base[NAMELEN];
+  RemovePath(base, infile);
+  strmcpy(q->name, base, NAMELEN - 1);
+  strmcpy(q->longname, base, DESCLEN - 1);
+  char input_format = 0;
+  ReadQueryFile(par, infile, input_format, par.wg, q, ali, g->pb, g->S, g->Sim);
+  PrepareQueryHMM(par, input_format, q, g->pc_hhm_context_engine, g->pc_hhm_context_mode, g->pb, g->R);
+  std::stringstream ss;
+  q->WriteToFile(ss, par.max_seqid, par.coverage, par.qid, par.Ndiff, par.qsc, 1, kArgv, g->pb);
+  par.gapb = gapb; par.pc_hhm_nocontext_mode = pcm;
+  delete ali; delete q;
+  const std::string s = ss.str();
+  if ((long)s.size() > cap) return -2;
+  memcpy(out, s.data(), s.size());
+  return (long)s.size();
+}
+
 // Read query HHM, add pseudocounts exactly like HHalign::run (src/hhalign.cpp:615-626), map to SIMD.
 int hhref_load_query_hhm(const char* path) {
   FILE* f = fopen(path, "r");
@@ -262,6 +301,26 @@ int hhref_prepare_template_hhm_raw(const char* path, int columnscore, float* p_r
   export_hmm(t, p_raw, tr, pav, nullptr, nullptr, nullptr, nullptr);
   t->IncludeNullModelInHMM(g->q, t, columnscore, par.half_window_size_local_aa_bg_freqs, g->pb);
   export_hmm(t, p_prep, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+  delete t;
+  return L;
+}
+
+// HMM::Read of a template file alone: Neff_HMM and has_pseudocounts as the reader leaves them; returns L (< 0: no
+// file).  The global pb, which the reader overwrites with the file's NULL line, is put back.
+extern "C" int hhref_read_hhm_header(const char* path, float* neff_hmm, int* has_pc) {
+  FILE* f = fopen(path, "r");
+  if (!f) return -1;
+  float pb[20];
+  memcpy(pb, g->pb, sizeof pb);
+  HMM* t = new HMM(MAXSEQDIS, g->maxres);
+  char pathbuf[NAMELEN];
+  Pathname(pathbuf, const_cast<char*>(path));
+  t->Read(f, g->par->maxcol, g->par->nseqdis, g->pb, pathbuf);
+  fclose(f);
+  memcpy(g->pb, pb, sizeof pb);
+  *neff_hmm = t->Neff_HMM;
+  *has_pc = t->has_pseudocounts ? 1 : 0;
+  const int L = t->L;
   delete t;
   return L;
 }
