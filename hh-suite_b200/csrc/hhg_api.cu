@@ -2726,7 +2726,13 @@ int hhg_comm_destroy(hhg_comm* c) {
 int hhg_comm_rank(const hhg_comm* c) { return c ? c->rank : 0; }
 int hhg_comm_world(const hhg_comm* c) { return c ? c->world : 1; }
 
+// Target id of the record that marks a rank's block in the exchange as refused (padding is -1).
+static constexpr int32_t kTopkRefused = -2;
+
 // Top-K of the last run of `plan`, merged over all ranks of `comm` (NULL / world 1: this GPU only).
+// Refusals are rank-symmetric: a rank whose input is bad still takes part in the ncclAllGather, with a block that
+// starts with a kTopkRefused record, and every rank refuses after the gather.  Refusing before the collective would
+// leave the other ranks waiting in it.
 static int plan_topk_impl(hhg_ctx* ctx, hhg_plan* pl, hhg_comm* comm, int K, int by_hit_score, const float* user_key,
                           int32_t id_base, const int32_t* global_ids, hhg_topk_rec* out, int* n_out) {
   static_assert(sizeof(hhg_topk_rec) == sizeof(TopkRec), "hhg_topk_rec / TopkRec layout");
@@ -2737,31 +2743,71 @@ static int plan_topk_impl(hhg_ctx* ctx, hhg_plan* pl, hhg_comm* comm, int K, int
   const int n = pl->n;
   const int world = comm ? comm->world : 1, rank = comm ? comm->rank : 0;
   const int kl = std::min(K, n);
+  // The key holds the global id as 32 bits above which nothing may wrap, and a NaN key has no place in the order.
+  // The loops that name the offending request run only on bad input.
+  char bad[192] = "";
+  if (global_ids) {
+    int32_t lo = 0;
+    for (int k = 0; k < n; ++k) lo = std::min(lo, global_ids[k]);
+    for (int k = 0; lo < 0 && !bad[0]; ++k)
+      if (global_ids[k] < 0) snprintf(bad, sizeof bad, "request %d: global id %d is negative", k, global_ids[k]);
+  } else if (id_base < 0 || (long long)id_base + n - 1 > INT32_MAX) {
+    snprintf(bad, sizeof bad, "global ids id_base + k = %d .. %lld leave [0, INT32_MAX]", id_base, (long long)id_base + n - 1);
+  }
+  if (user_key && !bad[0]) {
+    bool nan = false;
+    for (int k = 0; k < n; ++k) nan |= user_key[k] != user_key[k];
+    for (int k = 0; nan && !bad[0]; ++k)
+      if (std::isnan(user_key[k])) snprintf(bad, sizeof bad, "request %d: key is NaN", k);
+  }
+  if (bad[0] && world == 1) return fail(HHG_EINVAL, "hhg_plan_topk: %s", bad);
+  // More than min(K, n) keys at or below the K-th: two requests share a global id and tie on the value, so the
+  // emitted records would be whichever won the atomics.  Read back after the selection has run.
+  auto check_emitted = [&]() -> int {
+    unsigned int emitted = 0;
+    CK(cudaMemcpyAsync(&emitted, &pl->d_topk_state.p->out_count, sizeof emitted, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (emitted != (unsigned)kl)
+      snprintf(bad, sizeof bad, "%u requests rank at or above the %d-th: global ids are not unique", emitted, kl);
+    return HHG_OK;
+  };
   CK(pl->d_keys.ensure((size_t)n)); CK(pl->d_topk_state.ensure(1));
   CK(pl->d_topk_local.ensure((size_t)K)); CK(pl->d_topk_all.ensure((size_t)K * world));
-  if (global_ids) {
-    CK(pl->d_gids.ensure((size_t)n));
-    CK(cudaMemcpyAsync(pl->d_gids.p, global_ids, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  if (!bad[0]) {
+    if (global_ids) {
+      CK(pl->d_gids.ensure((size_t)n));
+      CK(cudaMemcpyAsync(pl->d_gids.p, global_ids, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    }
+    if (user_key) {
+      CK(pl->d_user_key.ensure((size_t)n));
+      CK(cudaMemcpyAsync(pl->d_user_key.p, user_key, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    }
+    TopkState init{};
+    init.krem = (unsigned)kl;
+    CK(cudaMemcpyAsync(pl->d_topk_state.p, &init, sizeof init, cudaMemcpyHostToDevice, st));
+    const int threads = 256, blocks = (n + threads - 1) / threads;
+    k_topk_keys<<<blocks, threads, 0, st>>>(n, pl->d_hits.p, by_hit_score, id_base, global_ids ? pl->d_gids.p : nullptr,
+                                              user_key ? pl->d_user_key.p : nullptr, pl->d_keys.p);
+    const int hblocks = std::min(blocks, ctx->sm_count * 4);
+    for (int p = 7; p >= 0; --p) {
+      k_topk_hist<<<hblocks, threads, 0, st>>>(n, pl->d_keys.p, p, pl->d_topk_state.p);
+      k_topk_scan<<<1, 256, 0, st>>>(pl->d_topk_state.p);
+    }
+    k_topk_emit<<<blocks, threads, 0, st>>>(n, pl->d_keys.p, pl->d_hits.p, rank, pl->d_topk_state.p, pl->d_topk_local.p, K);
+    ctx->launches += 18;
+    if (kl < K) { k_topk_pad<<<(K - kl + 255) / 256, 256, 0, st>>>(pl->d_topk_local.p, kl, K); ctx->launches++; }
+    CK(cudaGetLastError());
+    if (world > 1) {      // before the exchange, so that this rank's block can say so
+      const int rc = check_emitted();
+      if (rc != HHG_OK) return rc;
+    }
   }
-  if (user_key) {
-    CK(pl->d_user_key.ensure((size_t)n));
-    CK(cudaMemcpyAsync(pl->d_user_key.p, user_key, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  if (bad[0]) {
+    TopkRec r{};
+    r.target = kTopkRefused;
+    r.owner = rank;
+    CK(cudaMemcpyAsync(pl->d_topk_local.p, &r, sizeof r, cudaMemcpyHostToDevice, st));
   }
-  TopkState init{};
-  init.krem = (unsigned)kl;
-  CK(cudaMemcpyAsync(pl->d_topk_state.p, &init, sizeof init, cudaMemcpyHostToDevice, st));
-  const int threads = 256, blocks = (n + threads - 1) / threads;
-  k_topk_keys<<<blocks, threads, 0, st>>>(n, pl->d_hits.p, by_hit_score, id_base, global_ids ? pl->d_gids.p : nullptr,
-                                            user_key ? pl->d_user_key.p : nullptr, pl->d_keys.p);
-  const int hblocks = std::min(blocks, ctx->sm_count * 4);
-  for (int p = 7; p >= 0; --p) {
-    k_topk_hist<<<hblocks, threads, 0, st>>>(n, pl->d_keys.p, p, pl->d_topk_state.p);
-    k_topk_scan<<<1, 256, 0, st>>>(pl->d_topk_state.p);
-  }
-  k_topk_emit<<<blocks, threads, 0, st>>>(n, pl->d_keys.p, pl->d_hits.p, rank, pl->d_topk_state.p, pl->d_topk_local.p, K);
-  ctx->launches += 18;
-  if (kl < K) { k_topk_pad<<<(K - kl + 255) / 256, 256, 0, st>>>(pl->d_topk_local.p, kl, K); ctx->launches++; }
-  CK(cudaGetLastError());
   const TopkRec* src = pl->d_topk_local.p;
   if (world > 1) {
     NCK(g_nccl.AllGather(pl->d_topk_local.p, pl->d_topk_all.p, (size_t)K * sizeof(TopkRec), /*ncclChar*/ 0, comm->comm, st));
@@ -2770,10 +2816,24 @@ static int plan_topk_impl(hhg_ctx* ctx, hhg_plan* pl, hhg_comm* comm, int K, int
   std::vector<TopkRec> all((size_t)K * world);
   CK(cudaMemcpyAsync(all.data(), src, all.size() * sizeof(TopkRec), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  if (world == 1) {       // the stream is idle by now: no second wait on the selection
+    const int rc = check_emitted();
+    if (rc != HHG_OK) return rc;
+  }
+  if (bad[0]) return fail(HHG_EINVAL, "hhg_plan_topk: %s", bad);
+  for (int r = 0; r < world; ++r)
+    if (all[(size_t)r * K].target == kTopkRefused) return fail(HHG_EINVAL, "hhg_plan_topk: rank %d refused its input", r);
   // merge: keys are unique and totally ordered (score descending, global id ascending)
   all.erase(std::remove_if(all.begin(), all.end(), [](const TopkRec& r) { return r.target < 0; }), all.end());
   std::sort(all.begin(), all.end(), [](const TopkRec& a, const TopkRec& b) { return a.key < b.key; });
   const int m = (int)std::min<size_t>(all.size(), (size_t)K);
+  // a global id twice among the list and the record after it: held by two ranks (the record after the list catches
+  // their tie at the K-th place), or by two requests of one rank whose values differ
+  std::vector<int32_t> ids(std::min(all.size(), (size_t)m + 1));
+  for (size_t k = 0; k < ids.size(); ++k) ids[k] = all[k].target;
+  std::sort(ids.begin(), ids.end());
+  const auto dup = std::adjacent_find(ids.begin(), ids.end());
+  if (dup != ids.end()) return fail(HHG_EINVAL, "hhg_plan_topk: global id %d is in the list twice: global ids are not unique", *dup);
   memcpy(out, all.data(), (size_t)m * sizeof(TopkRec));
   *n_out = m;
   return HHG_OK;

@@ -37,17 +37,18 @@ __device__ __forceinline__ uint32_t orderable_f32(float f) {   // monotone incre
   return u ^ ((u >> 31) ? 0xFFFFFFFFu : 0x80000000u);
 }
 
-// user_key != NULL: caller-supplied ranking value per request, ASCENDING = better (e.g. the reference's score_aass)
+// user_key != NULL: caller-supplied ranking value per request, ASCENDING = better (e.g. the reference's score_aass).
+// The host has checked that every global id lies in [0, INT32_MAX] and that no caller key is NaN.
 __global__ void __launch_bounds__(256)
 k_topk_keys(int n, const HitRec* __restrict__ hits, int by_hit_score, int id_base, const int* __restrict__ gids,
             const float* __restrict__ user_key, unsigned long long* __restrict__ keys) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   const uint32_t gid = (uint32_t)(gids ? gids[k] : id_base + k);
-  uint32_t hi;
-  if (user_key) hi = orderable_f32(user_key[k]);
-  else hi = ~orderable_f32(by_hit_score ? hits[k].hit_score : hits[k].score);
-  keys[k] = ((unsigned long long)hi << 32) | gid;
+  float v = user_key ? user_key[k] : (by_hit_score ? hits[k].hit_score : hits[k].score);
+  if (v == 0.0f) v = 0.0f;      // -0.0 and +0.0 are one value: the global id breaks their tie like any other
+  const uint32_t o = orderable_f32(v);
+  keys[k] = ((unsigned long long)(user_key ? o : ~o) << 32) | gid;
 }
 
 // pass p (7 = most significant byte first): histogram byte p of the keys whose bytes above p equal the prefix
@@ -84,7 +85,8 @@ __global__ void k_topk_scan(TopkState* st) {
   st->hist[threadIdx.x] = 0;
 }
 
-// emit the records whose key is <= the K-th key (exactly K of them: keys are unique)
+// emit the records whose key is <= the K-th key: exactly K of them when keys are unique; the host reads out_count back
+// and refuses the call when two requests share a global id and their tie makes it larger
 __global__ void __launch_bounds__(256)
 k_topk_emit(int n, const unsigned long long* __restrict__ keys, const HitRec* __restrict__ hits, int owner,
             TopkState* st, TopkRec* __restrict__ out, int cap) {

@@ -493,8 +493,15 @@ float hhg_early_stop_sum(int n, const float* score, const int32_t* Lt, const flo
  *                        ascending), exchanges them with ONE ncclAllGather of K*56 bytes per rank and returns the
  *                        merged K best on every rank.  by_hit_score: 0 = raw Viterbi score, 1 = Hit.score.
  *                        Global id of request k = global_ids ? global_ids[k] : id_base + k  (host array of plan-n).
+ *                        Global ids must lie in [0, INT32_MAX] and be unique over all ranks; -0.0 and +0.0 are one
+ *                        value (their tie goes to the global id).  HHG_EINVAL, with nothing returned, when an id is
+ *                        negative, id_base + n - 1 exceeds INT32_MAX, a caller key is NaN, or two requests with one
+ *                        global id reach the list (both in it, or tied at the K-th place); a duplicate that ranks
+ *                        below the list on every rank does not change it and is not detected.  With world > 1 every
+ *                        rank refuses when any rank does: a rank with bad input still takes part in the exchange.
  *   hhg_plan_topk_paths: the state strings of the merged list (one ncclAllReduce of n_rec*width bytes; each row has
- *                        exactly one owner).  out[r*width ..] = path of recs[r], zero padded; width >= max nsteps. */
+ *                        exactly one owner).  out[r*width ..] = path of recs[r], zero padded; width >= max nsteps
+ *                        (a narrower width keeps the first width states of each path). */
 typedef struct hhg_comm hhg_comm;
 typedef struct hhg_topk_rec {
   int32_t target;   /* global target id                          */
