@@ -10,15 +10,18 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+HEADER = os.path.join(os.path.dirname(HERE), "include", "hhg.h")
 
 c_f32p = C.POINTER(C.c_float)
 c_i32p = C.POINTER(C.c_int32)
 c_i64p = C.POINTER(C.c_int64)
 c_u8p = C.POINTER(C.c_uint8)
+c_f64p = C.POINTER(C.c_double)
 
 
 class Params(C.Structure):
@@ -29,32 +32,6 @@ class Params(C.Structure):
 HIT_DTYPE = np.dtype([("score", np.float32), ("i2", np.int32), ("j2", np.int32), ("i1", np.int32),
                       ("j1", np.int32), ("nsteps", np.int32), ("matched_cols", np.int32),
                       ("path_off", np.int32), ("hit_score", np.float32), ("score_ss", np.float32)])
-
-SYMBOLS = ["hhg_last_error", "hhg_ctx_create", "hhg_ctx_destroy", "hhg_ctx_sync", "hhg_ctx_launch_count",
-           "hhg_db_create", "hhg_db_create_raw", "hhg_db_apply_null_model", "hhg_db_create_hhm", "hhg_hhm_scan", "hhg_hhm_parse",
-           "hhg_db_read_cols", "hhg_db_lengths", "hhg_db_read_pav", "hhg_db_create_packed", "hhg_debug_fastlog2_table", "hhg_db_destroy", "hhg_db_size", "hhg_db_columns", "hhg_query_set",
-           "hhg_viterbi_search", "hhg_plan_create", "hhg_plan_destroy", "hhg_plan_run", "hhg_plan_run_timed", "hhg_plan_fetch", "hhg_plan_hits_devptr",
-           "hhg_plan_cells", "hhg_plan_padded_cells", "hhg_plan_algorithmic_bytes", "hhg_plan_debug_bt",
-           "hhg_csdb_create", "hhg_csdb_destroy", "hhg_prefilter_ungapped", "hhg_prefilter_ungapped_run",
-           "hhg_prefilter_fetch", "hhg_prefilter_select", "hhg_log2lin", "hhg_mac_query_set", "hhg_mac_realign",
-           "hhg_mac_query_set_batch", "hhg_mac_realign_batch",
-           "hhg_mac_debug_posterior", "hhg_prefilter_build_profile", "hhg_prefilter_corrected_score",
-           "hhg_prefilter_sw", "hhg_prefilter_evalue", "hhg_prefilter_corrected_scores", "hhg_prefilter_evalues",
-           "hhg_comm_unique_id", "hhg_comm_create", "hhg_comm_destroy", "hhg_comm_rank", "hhg_comm_world",
-           "hhg_plan_topk", "hhg_plan_topk_by_key", "hhg_plan_topk_paths", "hhg_ctx_last_plan",
-           "hhg_hitlist_pvalues", "hhg_hitlist_hhblits_evalues", "hhg_hitlist_order", "hhg_early_stop_sum", "hhg_set_use_ss",
-           "hhg_query_set_batch", "hhg_viterbi_search_batch", "hhg_query_from_hhm",
-           "hhg_cs219_parse", "hhg_csdb_create_ffindex", "hhg_set_excluded_regions",
-           "hhg_msa_params_default", "hhg_a3m_scan", "hhg_a3m_parse", "hhg_msa_to_hmm", "hhg_db_create_a3m", "hhg_query_from_a3m",
-           "hhg_ca3m_scan", "hhg_ca3m_parse", "hhg_ca3m_to_hmm", "hhg_db_create_ca3m",
-           "hhg_crf_create", "hhg_crf_destroy", "hhg_crf_info", "hhg_query_context_pseudocounts", "hhg_crf_parse_host",
-           "hhg_crf_state", "hhg_crf_tail_host", "hhg_context_library_create", "hhg_context_library_parse_host",
-           "hhg_prefilter_ungapped_batch_run", "hhg_prefilter_ungapped_batch_fetch", "hhg_prefilter_select_batch",
-           "hhg_prefilter_sw_batch", "hhg_prefilter_batch_max_queries",
-           "hhg_dbstore_create", "hhg_dbstore_append_packed", "hhg_dbstore_append_db", "hhg_dbstore_destroy",
-           "hhg_dbstore_size", "hhg_dbstore_columns", "hhg_dbstore_lengths", "hhg_db_create_staged", "hhg_db_stage",
-           "hhg_db_staged_lookup", "hhg_recsrc_create_hhm", "hhg_recsrc_create_a3m", "hhg_recsrc_create_ca3m",
-           "hhg_recsrc_destroy", "hhg_recsrc_size", "hhg_db_create_staged_records", "hhg_db_staged_neff"]
 
 
 class PrepParams(C.Structure):
@@ -121,12 +98,12 @@ class Crf:
     def pc(self):
         out = np.zeros((self.n_states, 20), np.float64)
         n = np.zeros(1, np.int32); w = np.zeros(1, np.int32)
-        _ck(load().hhg_crf_info(self.h, _p(n, c_i32p), _p(w, c_i32p), out.ctypes.data))
+        _ck(load().hhg_crf_info(self.h, _p(n, c_i32p), _p(w, c_i32p), _p(out, c_f64p)))
         return out
 
     def state(self, k):
         w = np.zeros((self.window, 20), np.float64); b = C.c_double()
-        _ck(load().hhg_crf_state(self.h, k, w.ctypes.data, C.byref(b)))
+        _ck(load().hhg_crf_state(self.h, k, _p(w, c_f64p), C.byref(b)))
         return w, b.value
 
     def tail_host(self, score, f, neff_m, admix):
@@ -135,7 +112,7 @@ class Crf:
         score = np.ascontiguousarray(score, np.float64).copy()
         L = f.shape[0] - 2
         p = np.zeros((L + 2, 20), np.float32)
-        _ck(load().hhg_crf_tail_host(self.h, L, score.ctypes.data, _p(f, c_f32p), _p(neff_m, c_f32p), C.byref(admix), _p(p, c_f32p)))
+        _ck(load().hhg_crf_tail_host(self.h, L, _p(score, c_f64p), _p(f, c_f32p), _p(neff_m, c_f32p), C.byref(admix), _p(p, c_f32p)))
         return p
 
     def pseudocounts(self, f, neff_m, neff_hmm, pb, admix, want_pav=True):
@@ -209,6 +186,48 @@ def _p(a, t):
     return None if a is None else a.ctypes.data_as(t)
 
 
+def _norm_type(decl: str) -> str:
+    """A C type without const, one '*' per level of indirection: "const float* const*" -> "float**"."""
+    words = [w for w in re.findall(r"\w+|\*", decl) if w != "const"]
+    return " ".join(w for w in words if w != "*") + "*" * words.count("*")
+
+
+def _prototypes():
+    """(return type, name, [(parameter type, parameter name)]) of every hhg_* prototype in include/hhg.h."""
+    with open(HEADER) as f:
+        src = re.sub(r"/\*.*?\*/|//[^\n]*", " ", f.read(), flags=re.S)
+    protos = []
+    for ret, name, params in re.findall(r"([\w\s*]+?)\b(hhg_\w+)\s*\(([^()]*)\)\s*;", src):
+        args = [] if params.strip() in ("", "void") else [re.fullmatch(r"\s*(.*?)\b(\w+)\s*", p).groups()
+                                                            for p in params.split(",")]
+        protos.append((_norm_type(ret), name, [(_norm_type(t), a) for t, a in args]))
+    return protos
+
+
+PROTOTYPES = _prototypes()
+SYMBOLS = tuple(name for _, name, _ in PROTOTYPES)
+
+# The ctypes type of each C type in include/hhg.h.  Beyond these tables, hhg_<handle>** (the out-parameter of every
+# *_create) is POINTER(c_void_p) and any other pointer is c_void_p; any other type is refused.
+_ARGTYPES = {"int": C.c_int, "int32_t": C.c_int, "int64_t": C.c_int64, "long long": C.c_longlong, "size_t": C.c_size_t,
+             "float": C.c_float, "double": C.c_double, "float*": c_f32p, "int*": c_i32p, "int32_t*": c_i32p,
+             "int64_t*": c_i64p, "uint8_t*": c_u8p, "double*": c_f64p, "char*": C.c_char_p,
+             "hhg_params*": C.POINTER(Params), "hhg_prep_params*": C.POINTER(PrepParams),
+             "hhg_mac_params*": C.POINTER(MacParams)}
+_RESTYPES = {"int": C.c_int, "long long": C.c_longlong, "float": C.c_float, "double": C.c_double,
+             "char*": C.c_char_p, "void": None}
+
+
+def _ctypes_type(t: str, table: dict, what: str):
+    if t in table:
+        return table[t]
+    if re.fullmatch(r"hhg_\w+\*\*", t):
+        return C.POINTER(C.c_void_p)
+    if t.endswith("*"):
+        return C.c_void_p
+    raise HhgError(f"include/hhg.h: {what} has type '{t}', which the binding does not map")
+
+
 _lib = None
 
 
@@ -217,165 +236,18 @@ def lib_path() -> str:
 
 
 def load():
-    """Load libhhg.so (building it first if a toolchain is present). Never falls back to CPU code."""
+    """Load libhhg.so (building it first if a toolchain is present) and bind every prototype of include/hhg.h.
+    Never falls back to CPU code."""
     global _lib
     if _lib is not None:
         return _lib
     from . import build as _build
     path = os.environ.get("HHG_LIB") or _build.build()   # HHG_LIB: developer override (kernel variants)
     L = C.CDLL(path)
-    L.hhg_last_error.restype = C.c_char_p
-    L.hhg_ctx_create.argtypes = [C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
-    L.hhg_ctx_destroy.argtypes = [C.c_void_p]
-    L.hhg_ctx_sync.argtypes = [C.c_void_p]
-    L.hhg_ctx_launch_count.argtypes = [C.c_void_p]
-    L.hhg_ctx_launch_count.restype = C.c_longlong
-    L.hhg_db_create.argtypes = [C.c_void_p, C.c_int, c_i32p, c_i64p, c_i64p, c_i64p, c_f32p, c_f32p, c_u8p,
-                                C.POINTER(C.c_void_p)]
-    L.hhg_db_create_raw.argtypes = [C.c_void_p, C.c_int, c_i32p, c_i64p, c_i64p, c_i64p, c_f32p, c_f32p, c_u8p,
-                                    c_f32p, C.POINTER(C.c_void_p)]
-    L.hhg_db_apply_null_model.argtypes = [C.c_void_p, C.c_void_p, c_f32p, c_f32p, C.c_int]
-    L.hhg_db_create_hhm.argtypes = [C.c_void_p, C.c_int, C.c_char_p, c_i64p, c_i64p, C.POINTER(PrepParams), c_f32p,
-                                    C.POINTER(C.c_void_p)]
-    L.hhg_hhm_scan.argtypes = [C.c_char_p, C.c_int64, c_i32p, c_i32p]
-    L.hhg_db_read_cols.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_void_p]
-    L.hhg_hhm_parse.argtypes = [C.c_char_p, C.c_int64, C.c_int32, c_i32p, c_i32p, c_u8p, c_i32p, c_f32p, c_i32p]
-    L.hhg_db_lengths.argtypes = [C.c_void_p, c_i32p]
-    L.hhg_db_read_pav.argtypes = [C.c_void_p, C.c_void_p, c_f32p]
-    L.hhg_db_create_packed.argtypes = [C.c_void_p, C.c_int, c_i32p, C.c_void_p, C.c_int, c_f32p,
-                                       C.POINTER(C.c_void_p)]
-    L.hhg_debug_fastlog2_table.argtypes = [C.c_void_p, c_f32p]
-    L.hhg_db_destroy.argtypes = [C.c_void_p]
-    L.hhg_db_size.argtypes = [C.c_void_p]
-    L.hhg_db_columns.argtypes = [C.c_void_p]
-    L.hhg_db_columns.restype = C.c_longlong
-    L.hhg_query_set.argtypes = [C.c_void_p, C.c_int, c_f32p, c_f32p, c_u8p, c_f32p, C.POINTER(Params)]
-    L.hhg_viterbi_search.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, C.c_void_p, c_u8p, C.c_size_t,
-                                     c_i64p, c_i32p, c_i32p]
-    L.hhg_plan_create.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, C.POINTER(C.c_void_p)]
-    L.hhg_plan_destroy.argtypes = [C.c_void_p]
-    L.hhg_plan_run.argtypes = [C.c_void_p, C.c_void_p]
-    L.hhg_plan_run_timed.argtypes = [C.c_void_p, C.c_void_p, c_f32p, c_f32p]
-    L.hhg_plan_fetch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, c_u8p, C.c_size_t]
-    for f in ("hhg_plan_cells", "hhg_plan_padded_cells", "hhg_plan_algorithmic_bytes"):
-        getattr(L, f).argtypes = [C.c_void_p]
-        getattr(L, f).restype = C.c_double
-    L.hhg_plan_hits_devptr.argtypes = [C.c_void_p]
-    L.hhg_plan_hits_devptr.restype = C.c_void_p
-    L.hhg_plan_debug_bt.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_u8p]
-    L.hhg_csdb_create.argtypes = [C.c_void_p, C.c_int, c_i32p, c_i64p, c_u8p, C.POINTER(C.c_void_p)]
-    L.hhg_csdb_destroy.argtypes = [C.c_void_p]
-    L.hhg_prefilter_ungapped.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_u8p, C.c_int, c_i32p]
-    L.hhg_prefilter_ungapped_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_u8p, C.c_int, C.c_int]
-    L.hhg_prefilter_select.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, c_i32p, c_i32p,
-                                       C.c_int, c_i32p]
-    L.hhg_log2lin.argtypes = [C.c_int64, c_f32p, c_f32p]
-    L.hhg_mac_query_set.argtypes = [C.c_void_p, C.c_int, c_f32p, c_f32p]
-    L.hhg_mac_realign.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, c_i32p, c_i64p, c_i32p, c_i32p, c_i64p,
-                                  c_i32p, c_i32p, C.POINTER(MacParams), C.c_void_p, c_i32p, c_i32p, c_u8p, c_f32p,
-                                  C.c_size_t]
-    L.hhg_mac_query_set_batch.argtypes = [C.c_void_p, C.c_int, c_i32p, C.c_void_p, C.c_void_p, c_f32p]
-    L.hhg_mac_realign_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, c_i32p, c_i32p, c_i64p, c_i32p, c_i32p,
-                                        c_i64p, c_i32p, c_i32p, C.c_int, c_f32p, C.POINTER(MacParams), C.c_void_p,
-                                        c_i32p, c_i32p, c_u8p, c_f32p, C.c_size_t]
-    L.hhg_mac_debug_posterior.argtypes = [C.c_void_p, C.c_int, c_f32p]
-    L.hhg_prefilter_fetch.argtypes = [C.c_void_p, C.c_void_p, c_i32p]
-    L.hhg_prefilter_build_profile.argtypes = [C.c_int, c_f32p, c_f32p, c_f32p, C.c_int, C.c_int, c_u8p]
-    L.hhg_prefilter_corrected_score.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
-    L.hhg_prefilter_evalue.argtypes = [C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_int]
-    L.hhg_prefilter_evalue.restype = C.c_double
-    L.hhg_prefilter_corrected_scores.argtypes = [C.c_int, c_i32p, c_i32p, C.c_int, C.c_int, c_i32p]
-    L.hhg_prefilter_evalues.argtypes = [C.c_int, c_i32p, c_i32p, C.c_longlong, C.c_int, C.c_int,
-                                        C.POINTER(C.c_double)]
-    L.hhg_prefilter_sw.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, C.c_int, c_u8p, C.c_int, C.c_int, C.c_int,
-                                   c_i32p]
-    L.hhg_prefilter_ungapped_batch_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, C.POINTER(C.c_void_p),
-                                                   C.c_int]
-    L.hhg_prefilter_ungapped_batch_fetch.argtypes = [C.c_void_p, C.c_void_p, c_i32p]
-    L.hhg_prefilter_batch_max_queries.argtypes = [C.c_void_p, C.c_void_p]
-    L.hhg_prefilter_select_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, c_i32p,
-                                             c_i32p, C.c_int, c_i32p]
-    L.hhg_prefilter_sw_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, C.POINTER(C.c_void_p), C.c_int, c_i32p,
-                                         c_i32p, C.c_int, C.c_int, C.c_int, c_i32p]
-    L.hhg_comm_unique_id.argtypes = [C.c_void_p]
-    L.hhg_comm_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
-    L.hhg_comm_destroy.argtypes = [C.c_void_p]
-    L.hhg_comm_rank.argtypes = [C.c_void_p]
-    L.hhg_comm_world.argtypes = [C.c_void_p]
-    L.hhg_plan_topk.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int32, c_i32p, C.c_void_p,
-                                c_i32p]
-    L.hhg_plan_topk_by_key.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, c_f32p, C.c_int32, c_i32p, C.c_void_p,
-                                       c_i32p]
-    L.hhg_hitlist_pvalues.argtypes = [C.c_int, c_f32p, c_f32p, c_i32p, c_f32p, c_i32p, C.c_int, C.c_float, C.c_int,
-                                      C.c_int, C.c_int, C.c_float, C.c_void_p]
-    L.hhg_hitlist_hhblits_evalues.argtypes = [C.c_int, C.c_void_p, c_f32p, C.c_float, C.c_int, C.c_float, C.c_float,
-                                              C.c_float, C.c_double]
-    L.hhg_hitlist_order.argtypes = [C.c_int, C.c_void_p, C.c_void_p, c_i32p]
-    L.hhg_early_stop_sum.argtypes = [C.c_int, c_f32p, c_i32p, c_f32p, C.c_int, C.c_float, C.c_int, C.c_int, C.c_float,
-                                     C.c_float, C.c_float, C.c_double]
-    L.hhg_early_stop_sum.restype = C.c_float
-    L.hhg_set_use_ss.argtypes = [C.c_void_p, C.c_int]
-    L.hhg_query_from_hhm.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.POINTER(PrepParams), c_f32p, C.c_int32, c_i32p,
-                                     c_f32p, c_f32p, c_u8p, c_f32p, c_f32p]
-    L.hhg_msa_params_default.argtypes = [C.c_void_p]
-    L.hhg_msa_params_default.restype = None
-    L.hhg_a3m_scan.argtypes = [C.c_char_p, C.c_int64, C.c_void_p, c_i32p, c_i32p, c_i32p]
-    L.hhg_a3m_parse.argtypes = [C.c_char_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32, c_i32p, c_u8p, C.c_void_p,
-                                C.c_void_p, c_i32p, c_i32p]
-    L.hhg_msa_to_hmm.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_void_p, c_f32p, c_f32p, C.c_int32, C.c_int32,
-                                 c_i32p, C.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_u8p]
-    L.hhg_crf_create.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.POINTER(C.c_void_p)]
-    L.hhg_crf_parse_host.argtypes = [C.c_char_p, C.c_int64, C.POINTER(C.c_void_p)]
-    L.hhg_crf_destroy.argtypes = [C.c_void_p]
-    L.hhg_crf_info.argtypes = [C.c_void_p, c_i32p, c_i32p, C.c_void_p]
-    L.hhg_crf_state.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_double)]
-    L.hhg_crf_tail_host.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, c_f32p, c_f32p, C.c_void_p, c_f32p]
-    L.hhg_context_library_create.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_double, C.c_double, C.POINTER(C.c_void_p)]
-    L.hhg_context_library_parse_host.argtypes = [C.c_char_p, C.c_int64, C.c_double, C.c_double, C.POINTER(C.c_void_p)]
-    L.hhg_query_context_pseudocounts.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, c_f32p, c_f32p, C.c_float, c_f32p,
-                                                 C.c_void_p, c_f32p, c_f32p]
-    L.hhg_ca3m_scan.argtypes = [C.c_char_p, C.c_int64, C.c_void_p, C.c_void_p, c_i32p, c_i32p]
-    L.hhg_ca3m_parse.argtypes = [C.c_char_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, c_i32p, c_u8p,
-                                 C.c_void_p, C.c_void_p, c_i32p, c_i32p]
-    L.hhg_ca3m_to_hmm.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_void_p, C.c_void_p, c_f32p, c_f32p, C.c_int32,
-                                  C.c_int32, c_i32p, C.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p]
-    L.hhg_db_create_ca3m.argtypes = [C.c_void_p, C.c_int, C.c_char_p, c_i64p, c_i64p, C.c_void_p, C.c_void_p, c_f32p, c_f32p,
-                                     C.POINTER(PrepParams), c_f32p, C.POINTER(C.c_void_p)]
-    L.hhg_query_from_a3m.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_void_p, c_f32p, c_f32p, C.POINTER(PrepParams),
-                                     c_f32p, C.c_int32, c_i32p, c_f32p, c_f32p, c_u8p, c_f32p, c_f32p]
-    L.hhg_db_create_a3m.argtypes = [C.c_void_p, C.c_int, C.c_char_p, c_i64p, c_i64p, C.c_void_p, c_f32p, c_f32p,
-                                    C.POINTER(PrepParams), c_f32p, C.POINTER(C.c_void_p)]
-    L.hhg_set_excluded_regions.argtypes = [C.c_void_p, C.c_int, c_i32p, c_i32p, C.c_int, c_i32p, c_i32p]
-    L.hhg_cs219_parse.argtypes = [C.c_char_p, C.c_int64, c_f32p, C.c_int, c_i32p]
-    L.hhg_csdb_create_ffindex.argtypes = [C.c_void_p, C.c_int, C.c_char_p, c_i64p, c_i64p, C.POINTER(C.c_void_p)]
-    L.hhg_query_set_batch.argtypes = [C.c_void_p, C.c_int, c_i32p, C.c_void_p, C.c_void_p, C.c_void_p, c_f32p, c_f32p,
-                                      C.POINTER(Params)]
-    L.hhg_viterbi_search_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, c_i32p, C.c_int, c_f32p, C.c_void_p,
-                                           c_u8p, C.c_size_t, c_i64p, c_i32p, c_i32p]
-    L.hhg_plan_topk_paths.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, c_u8p]
-    L.hhg_ctx_last_plan.argtypes = [C.c_void_p]
-    L.hhg_ctx_last_plan.restype = C.c_void_p
-    L.hhg_dbstore_create.argtypes = [C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.POINTER(C.c_void_p)]
-    L.hhg_dbstore_append_packed.argtypes = [C.c_void_p, C.c_int, c_i32p, C.c_void_p, c_f32p]
-    L.hhg_dbstore_append_db.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    L.hhg_dbstore_destroy.argtypes = [C.c_void_p]
-    L.hhg_dbstore_size.argtypes = [C.c_void_p]
-    L.hhg_dbstore_columns.argtypes = [C.c_void_p]
-    L.hhg_dbstore_columns.restype = C.c_longlong
-    L.hhg_dbstore_lengths.argtypes = [C.c_void_p, c_i32p]
-    L.hhg_db_create_staged.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.POINTER(C.c_void_p)]
-    L.hhg_db_stage.argtypes = [C.c_void_p, C.c_void_p, C.c_int, c_i32p, c_i32p, C.c_void_p]
-    L.hhg_db_staged_lookup.argtypes = [C.c_void_p, C.c_int, c_i32p, c_i32p, c_i64p]
-    L.hhg_recsrc_create_hhm.argtypes = [C.c_void_p, C.c_int, C.c_char_p, c_i64p, c_i64p, C.POINTER(PrepParams), c_f32p,
-                                        C.c_int, C.POINTER(C.c_void_p)]
-    L.hhg_recsrc_create_a3m.argtypes = [C.c_void_p, C.c_int, C.c_char_p, c_i64p, c_i64p, C.c_void_p, c_f32p, c_f32p,
-                                        C.POINTER(PrepParams), c_f32p, C.c_int, C.POINTER(C.c_void_p)]
-    L.hhg_recsrc_create_ca3m.argtypes = [C.c_void_p, C.c_int, C.c_char_p, c_i64p, c_i64p, C.c_void_p, C.c_void_p, c_f32p,
-                                         c_f32p, C.POINTER(PrepParams), c_f32p, C.c_int, C.POINTER(C.c_void_p)]
-    L.hhg_recsrc_destroy.argtypes = [C.c_void_p]
-    L.hhg_recsrc_size.argtypes = [C.c_void_p]
-    L.hhg_db_create_staged_records.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.POINTER(C.c_void_p)]
-    L.hhg_db_staged_neff.argtypes = [C.c_void_p, C.c_int, c_i32p, c_f32p]
+    for ret, name, params in PROTOTYPES:
+        fn = getattr(L, name)
+        fn.restype = _ctypes_type(ret, _RESTYPES, f"the return value of {name}")
+        fn.argtypes = [_ctypes_type(t, _ARGTYPES, f"parameter {a} of {name}") for t, a in params]
     _lib = L
     return L
 

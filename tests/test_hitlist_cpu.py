@@ -10,32 +10,24 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "hitlist_v1.npz")
 
-STATS = np.dtype([("Pval", np.float64), ("logPval", np.float64), ("Eval", np.float64), ("logEval", np.float64),
-                  ("score_aass", np.float32), ("Probab", np.float32), ("lamda", np.float32), ("mu", np.float32)])
-
 
 def product_stats(score, score_ss, L, neff, qL, qneff, N, loc, ssm, ssw, ssm2=None, files=None, hhblits=None):
     import hhsuite_b200 as hh
     lib = hh.capi.load()
     n = len(score)
-    out = np.zeros(n, STATS)
+    out = np.zeros(n, hh.capi.STATS_DTYPE)
     f32 = lambda a: np.ascontiguousarray(a, np.float32)   # noqa: E731
     i32 = lambda a: None if a is None else np.ascontiguousarray(a, np.int32)   # noqa: E731
     p = hh.capi._p
     s, ss, Lt, ne, s2 = f32(score), f32(score_ss), i32(L), f32(neff), i32(ssm2)
-    lib.hhg_hitlist_pvalues.argtypes = [C.c_int, hh.capi.c_f32p, hh.capi.c_f32p, hh.capi.c_i32p, hh.capi.c_f32p,
-                                        hh.capi.c_i32p, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]
     assert lib.hhg_hitlist_pvalues(n, p(s, hh.capi.c_f32p), p(ss, hh.capi.c_f32p), p(Lt, hh.capi.c_i32p),
                                    p(ne, hh.capi.c_f32p), p(s2, hh.capi.c_i32p), qL, qneff, N, loc, ssm, ssw,
                                    out.ctypes.data_as(C.c_void_p)) == 0
     if hhblits:
-        lib.hhg_hitlist_hhblits_evalues.argtypes = [C.c_int, C.c_void_p, hh.capi.c_f32p, C.c_float, C.c_int, C.c_float,
-                                                    C.c_float, C.c_float, C.c_double]
         assert lib.hhg_hitlist_hhblits_evalues(n, out.ctypes.data_as(C.c_void_p), p(ne, hh.capi.c_f32p), qneff,
                                                hhblits["dbsize"], 0.4, 0.02, 0.1, hhblits["thresh"]) == 0
     order = np.zeros(n, np.int32)
     farr = None if files is None else (C.c_char_p * n)(*[f.encode() for f in files])
-    lib.hhg_hitlist_order.argtypes = [C.c_int, C.c_void_p, C.c_void_p, hh.capi.c_i32p]
     assert lib.hhg_hitlist_order(n, out.ctypes.data_as(C.c_void_p), farr, p(order, hh.capi.c_i32p)) == 0
     return out, order
 
