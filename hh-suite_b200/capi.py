@@ -290,6 +290,11 @@ class Context:
         _ck(self.L.hhg_set_excluded_regions(self.h, len(q), _p(ql, c_i32p), _p(qh, c_i32p), len(t), _p(tl, c_i32p),
                                             _p(th, c_i32p)))
 
+    def set_scwin(self, half_window: int):
+        """-scwin: the half window D of column score 5 (the local amino-acid composition correction) for every following
+        call of this context that applies it; default 40, D >= 1."""
+        _ck(self.L.hhg_set_scwin(self.h, int(half_window)))
+
     def set_query(self, p, tr, ss=None, S33=None, local=True, egq=0.0, egt=0.0, shift=-0.03, ssw=0.11,
                   use_ss=False, corr=0.1, ssm=2):
         p = np.ascontiguousarray(p, np.float32); tr = np.ascontiguousarray(tr, np.float32)
@@ -301,6 +306,17 @@ class Context:
         _ck(self.L.hhg_query_set(self.h, Lq, _p(p, c_f32p), _p(tr, c_f32p), _p(ss, c_u8p), _p(S33, c_f32p),
                                  C.byref(par)))
         self.Lq = Lq
+
+
+def query_local_background(ctx, p, pb):
+    """Column score 5 for a query (PrepareQueryHMM under -sc 5): HMM::p [(L+2), 20] divided, rows 1..L, by the square
+    root of its local background with the context's half window (Context.set_scwin) and the background pb[20].  Returns
+    a new array; rows 0 and L+1 are copied unchanged."""
+    out = np.array(p, np.float32, copy=True, order="C")
+    pb = np.ascontiguousarray(pb, np.float32)
+    assert out.ndim == 2 and out.shape[1] == 20 and pb.shape == (20,)
+    _ck(ctx.L.hhg_query_local_background(ctx.h, out.shape[0] - 2, _p(pb, c_f32p), _p(out, c_f32p)))
+    return out
 
 
 def log2lin(tr):
@@ -394,7 +410,9 @@ def mac_realign(ctx, db, targets, vits, excl=None, local=True, shift=-0.03, mact
 def mac_realign_batch(ctx, db, req_query, targets, vits, excl=None, columnscore=1, pb=None, local=True, shift=-0.03,
                       mact=0.35):
     """hhg_mac_realign_batch: request r realigns query req_query[r] of the last mac_query_set_batch against
-    targets[r]; vits / excl and the result as in mac_realign.  columnscore / pb: the null model of a raw shard."""
+    targets[r]; vits / excl and the result as in mac_realign.  columnscore / pb: the null model of a raw shard (5: the
+    local composition correction with the context's half window, applied to a copy; the queries divided by
+    query_local_background)."""
     n = len(targets)
     rq = np.ascontiguousarray(req_query, np.int32); targets = np.ascontiguousarray(targets, np.int32)
     vit, voff, vi, vj, eoff, ei, ej = _mac_inputs(vits, excl)
@@ -661,6 +679,8 @@ class TargetDB:
         return out
 
     def apply_null_model(self, q_pav=None, pb=None, columnscore=1):
+        """HMM::IncludeNullModelInHMM on the raw records: columnscore 0 pb, 1 (q_pav + t.pav)/2, 2 t.pav, 3 q_pav,
+        5 the local composition correction (pb and the context's half window; q_pav is not used)."""
         q_pav = None if q_pav is None else np.ascontiguousarray(q_pav, np.float32)
         pb = None if pb is None else np.ascontiguousarray(pb, np.float32)
         _ck(self.ctx.L.hhg_db_apply_null_model(self.ctx.h, self.h, _p(q_pav, c_f32p), _p(pb, c_f32p), columnscore))
@@ -1047,7 +1067,9 @@ def query_set_batch(ctx: Context, queries, S33=None, q_pav=None, local=True, egq
 def viterbi_search_batch(ctx: Context, db: TargetDB, req_query, ids, columnscore=1, pb=None, want_paths=True,
                          exclusions=None):
     """hhg_viterbi_search_batch: request k aligns query req_query[k] of the current batch with target ids[k].
-    exclusions: optional list (per request) of (i_steps, j_steps) int arrays to mask, as in viterbi_search."""
+    exclusions: optional list (per request) of (i_steps, j_steps) int arrays to mask, as in viterbi_search.
+    columnscore 5 over a raw shard divides the named targets in the shard itself and leaves it unprepared (apply_null_model
+    again before a single-query search); the queries must be divided by query_local_background."""
     rq = np.ascontiguousarray(req_query, np.int32); ids = np.ascontiguousarray(ids, np.int32)
     n = len(ids)
     hits = np.zeros(n, HIT_DTYPE)

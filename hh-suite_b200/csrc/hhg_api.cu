@@ -7,6 +7,7 @@
 #include "hhg_msa.cuh"
 #include "hhg_crf.cuh"
 #include "hhg_mac.cuh"
+#include "hhg_localbg.cuh"
 #include "hhg_topk.cuh"
 #include "hhg_hitlist.h"
 #include "hhg_stage_cache.h"
@@ -137,7 +138,10 @@ struct hhg_ctx {
   std::vector<float> h_q_pav;
   bool has_q_pav = false;
   DevBuf<float> d_q_pav, d_pb;
-  float h_pb[20] = {};   // host copy of d_pb (the background of columnscore 0 in the last batch search)
+  float h_pb[20] = {};   // host copy of d_pb (the background of columnscore 0 and 5 in the last batch search)
+  int scwin = 40;        // half window D of columnscore 5 (par.half_window_size_local_aa_bg_freqs, -scwin)
+  DevBuf<LocalBgSeg> lbg_seg;   // k_local_bg's segments and background of the last call
+  DevBuf<float> lbg_pb;
   // excluded regions (-excl / -template_excl), applied to every search until cleared: ex = {q_lo[ex_nq], q_hi[ex_nq],
   // t_lo[ex_nt], t_hi[ex_nt]} as k_celloff_regions and k_mac_realign read it from d_ex
   std::vector<int> ex;
@@ -291,10 +295,12 @@ struct hhg_plan {
   std::vector<int2> items;
   long long jc_total = 0;                 // float4 in the job-interleaved operand stream
   unsigned long long jc_version = 0;      // db->cols_version the stream was built from (0 = never)
-  int nm_mode = -1;                       // >= 0: columnscore of the null model fused into the stream (raw shard)
+  int nm_mode = -1;                       // 0..3: columnscore of the null model fused into the stream (raw shard);
+                                          // 5: cols of the plan's targets hold the local composition correction
   int jc_nm_mode = -2;                    // nm_mode / query batch the stream was built with
   unsigned long long jc_query_serial = 0;
-  float jc_pb[20] = {};                   // pb the stream was divided by (nm_mode 0)
+  float jc_pb[20] = {};                   // pb the stream was divided by (nm_mode 0 and 5)
+  int jc_scwin = 0;                       // half window of the local composition correction (nm_mode 5)
   std::vector<Wave> waves;
   long long path_total = 0;
   // device
@@ -412,6 +418,52 @@ static int ctx_aux_stream(hhg_ctx* ctx) {
   CK(cudaStreamCreateWithFlags(&ctx->aux_stream, cudaStreamNonBlocking));
   CK(cudaEventCreateWithFlags(&ctx->aux_ev[0], cudaEventDisableTiming));
   CK(cudaEventCreateWithFlags(&ctx->aux_ev[1], cudaEventDisableTiming));
+  return HHG_OK;
+}
+
+// Columnscore 5: one k_local_bg launch over `segs` (records src -> dst, two different buffers) with the context's
+// half window and the background pb[20] (host), queued on the context stream.  The host vectors may go when it returns.
+static int local_bg_launch(hhg_ctx* ctx, const std::vector<LocalBgSeg>& segs, const float4* src, float4* dst,
+                           const float* pb) {
+  if (segs.empty()) return HHG_OK;
+  if ((const void*)src == (const void*)dst) return fail(HHG_EINVAL, "k_local_bg: source and destination are one buffer");
+  CK(ctx->lbg_seg.ensure(segs.size()));
+  CK(ctx->lbg_pb.ensure(20));
+  CK(cudaMemcpyAsync(ctx->lbg_seg.p, segs.data(), segs.size() * sizeof(LocalBgSeg), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->lbg_pb.p, pb, 20 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  const int warps = kLocalBgThreads / 32;
+  const long long blocks = std::min<long long>(((long long)segs.size() + warps - 1) / warps, (long long)ctx->sm_count * 8);
+  k_local_bg<<<(unsigned)blocks, kLocalBgThreads, 0, ctx->stream>>>((int)segs.size(), ctx->lbg_seg.p,
+                                                                     reinterpret_cast<const float*>(src),
+                                                                     reinterpret_cast<float*>(dst), ctx->lbg_pb.p,
+                                                                     ctx->scwin);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  return HHG_OK;
+}
+
+int hhg_set_scwin(hhg_ctx* ctx, int half_window) {
+  if (!ctx) return fail(HHG_EINVAL, "ctx is NULL");
+  if (half_window < 1) return fail(HHG_EINVAL, "hhg_set_scwin: half window %d < 1", half_window);
+  ctx->scwin = half_window;
+  return HHG_OK;
+}
+
+int hhg_query_local_background(hhg_ctx* ctx, int L, const float* pb, float* p) {
+  if (!ctx || !pb || !p) return fail(HHG_EINVAL, "hhg_query_local_background: bad argument");
+  if (L < 1 || L > 32767) return fail(HHG_EINVAL, "hhg_query_local_background: query length %d out of [1,32767]", L);
+  CK(cudaSetDevice(ctx->device));
+  std::vector<float> rec((size_t)L * kRecFloats, 0.f);
+  for (int i = 1; i <= L; ++i) memcpy(&rec[(size_t)(i - 1) * kRecFloats], p + (size_t)i * 20, 80);
+  DevBuf<float4> d_src, d_dst;
+  CK(d_src.alloc((size_t)L * 7));
+  CK(d_dst.alloc((size_t)L * 7));
+  CK(cudaMemcpyAsync(d_src.p, rec.data(), rec.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  const int rc = local_bg_launch(ctx, {LocalBgSeg{0, 0, L, 0}}, d_src.p, d_dst.p, pb);
+  if (rc != HHG_OK) return rc;
+  CK(cudaMemcpyAsync(rec.data(), d_dst.p, rec.size() * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  for (int i = 1; i <= L; ++i) memcpy(p + (size_t)i * 20, &rec[(size_t)(i - 1) * kRecFloats], 80);
   return HHG_OK;
 }
 
@@ -556,10 +608,23 @@ int hhg_db_create_raw(hhg_ctx* ctx, int n, const int32_t* L, const int64_t* p_of
 
 int hhg_db_apply_null_model(hhg_ctx* ctx, hhg_db* db, const float* q_pav, const float* pb, int columnscore) {
   if (!ctx || !db || !db->raw) return fail(HHG_EINVAL, "hhg_db_apply_null_model: db was not created raw");
-  if (columnscore < 0 || columnscore > 3) return fail(HHG_EINVAL, "columnscore %d not supported (0..3)", columnscore);
+  if (columnscore < 0 || columnscore == 4 || columnscore > 5)
+    return fail(HHG_EINVAL, "columnscore %d not supported (0..3, 5)", columnscore);
   if ((columnscore == 1 || columnscore == 3) && !q_pav) return fail(HHG_EINVAL, "q_pav is NULL");
-  if (columnscore == 0 && !pb) return fail(HHG_EINVAL, "pb is NULL");
+  if ((columnscore == 0 || columnscore == 5) && !pb) return fail(HHG_EINVAL, "pb is NULL");
   CK(cudaSetDevice(ctx->device));
+  if (columnscore == 5) {
+    // query-independent: every target (every occupied slot of a staged shard) divided in place of cols
+    std::vector<LocalBgSeg> segs;
+    for (int k = 0; k < db->n; ++k)
+      if (db->L[k] > 0) segs.push_back(LocalBgSeg{db->col_off[k], db->col_off[k], db->L[k], 0});
+    const int rc = local_bg_launch(ctx, segs, db->cols_raw.p, db->cols.p, pb);
+    if (rc != HHG_OK) return rc;
+    CK(cudaStreamSynchronize(ctx->stream));
+    db->prepared = true;
+    db->cols_version++;
+    return HHG_OK;
+  }
   DevBuf<float> dq;
   CK(dq.alloc(40));
   float h[40] = {0};
@@ -2426,9 +2491,13 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
   if (pl->q_L != ctx->q_L || pl->q_row0 != ctx->q_row0) return fail(HHG_EINVAL, "plan was made for another query (batch) geometry");
   const hhg_db* db = pl->db;
   if (pl->db_serial != db->serial) return fail(HHG_EINVAL, "hhg_plan_run: the shard was staged anew after the plan was made");
-  const bool fused = pl->nm_mode >= 0;     // null model factored in per job while the operand stream is built
+  // nm_mode 0..3: null model factored in per job while the operand stream is built; 5: the batch search divided the
+  // `cols` of this plan's targets (k_local_bg) just before, the rest of the shard may be unprepared
+  const bool fused = pl->nm_mode >= 0 && pl->nm_mode != 5;
+  const int div_mode = fused ? pl->nm_mode : -1;
   if (fused && (!db->raw || !ctx->has_q_pav)) return fail(HHG_EINVAL, "fused null model needs a raw shard and query pav");
-  if (!fused && !db->prepared) return fail(HHG_EINVAL, "raw db: call hhg_db_apply_null_model for the current query first");
+  if (!fused && pl->nm_mode != 5 && !db->prepared)
+    return fail(HHG_EINVAL, "raw db: call hhg_db_apply_null_model for the current query first");
   if (ctx->par.use_ss && (!db->has_ss || !ctx->has_ss || !ctx->has_S33))
     return fail(HHG_EINVAL, "use_ss requested but query/db/S33 carry no ss information");
   CK(cudaSetDevice(ctx->device));
@@ -2445,7 +2514,8 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
   CK(cudaMemsetAsync(pl->d_counter.p, 0, pl->waves.size() * 4, st));
   if (pl->jc_version != db->cols_version || pl->jc_nm_mode != pl->nm_mode ||
       (fused && pl->jc_query_serial != ctx->query_serial) ||
-      (pl->nm_mode == 0 && memcmp(pl->jc_pb, ctx->h_pb, sizeof pl->jc_pb) != 0)) {
+      ((pl->nm_mode == 0 || pl->nm_mode == 5) && memcmp(pl->jc_pb, ctx->h_pb, sizeof pl->jc_pb) != 0) ||
+      (pl->nm_mode == 5 && pl->jc_scwin != ctx->scwin)) {
     // (re)build the job-interleaved operand stream: once per plan, again after every hhg_db_apply_null_model (the
     // prepared emissions changed) and, with the fused null model, for every new query batch and, with columnscore 0,
     // for every new pb (k_backtrace divides by the current one, so the forward pass must too)
@@ -2453,7 +2523,7 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
     for (const JobDesc& jd : pl->jobs) maxL = std::max(maxL, jd.Lmax);
     dim3 grid((unsigned)pl->njobs, (unsigned)std::min(64, (maxL + 7) / 8), 1);
     k_interleave_cols<<<grid, 256, 0, st>>>(pl->d_jobs.p, pl->d_job_target.p, fused ? db->cols_raw.p : db->cols.p,
-                                            db->dcol_off.p, db->dL.p, pl->d_jcols.p, pl->nm_mode, ctx->d_q_pav.p,
+                                            db->dcol_off.p, db->dL.p, pl->d_jcols.p, div_mode, ctx->d_q_pav.p,
                                             db->pav.p, ctx->d_pb.p);
     ctx->launches++;
     CK(cudaGetLastError());
@@ -2461,6 +2531,7 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
     pl->jc_nm_mode = pl->nm_mode;
     pl->jc_query_serial = ctx->query_serial;
     memcpy(pl->jc_pb, ctx->h_pb, sizeof pl->jc_pb);
+    pl->jc_scwin = ctx->scwin;
   }
   for (size_t wi = 0; wi < pl->waves.size(); ++wi) {
     const Wave& w = pl->waves[wi];
@@ -2495,7 +2566,7 @@ static int plan_run_impl(hhg_ctx* ctx, hhg_plan* pl, bool timed) {
     BtParams B{};
     B.n_req = pl->n;   // filtered by job range inside: simpler to launch per wave over all requests
     B.jobs = pl->d_jobs.p; B.reqs = pl->d_reqs.p;
-    B.nm_mode = pl->nm_mode; B.q_pav = ctx->d_q_pav.p; B.t_pav = db->pav.p; B.pb = ctx->d_pb.p;
+    B.nm_mode = div_mode; B.q_pav = ctx->d_q_pav.p; B.t_pav = db->pav.p; B.pb = ctx->d_pb.p;
     B.bt = pl->d_bt.p; B.strip_score = pl->d_strip_score.p; B.strip_ij = pl->d_strip_ij.p;
     B.hits = pl->d_hits.p; B.paths = pl->d_paths.p;
     B.job_begin = w.job_begin; B.job_end = w.job_end;
@@ -2618,6 +2689,14 @@ int hhg_viterbi_search_batch(hhg_ctx* ctx, const hhg_db* db, int n, const int32_
                              int columnscore, const float* pb, hhg_hit* hits, uint8_t* paths, size_t paths_cap,
                              const int64_t* excl_off, const int32_t* excl_i, const int32_t* excl_j) {
   if (!ctx || !db || !req_query || !ids) return fail(HHG_EINVAL, "hhg_viterbi_search_batch: bad argument");
+  if (db->raw) {
+    if (columnscore < 0 || columnscore == 4 || columnscore > 5)
+      return fail(HHG_EINVAL, "hhg_viterbi_search_batch: columnscore %d", columnscore);
+    if (columnscore != 5 && !ctx->has_q_pav)
+      return fail(HHG_EINVAL, "hhg_viterbi_search_batch: raw shard needs q_pav in hhg_query_set_batch");
+    if ((columnscore == 0 || columnscore == 5) && !pb)
+      return fail(HHG_EINVAL, "hhg_viterbi_search_batch: columnscore %d needs pb", columnscore);
+  }
   if (!ctx->scratch_plan) ctx->scratch_plan = new hhg_plan();
   hhg_plan* pl = ctx->scratch_plan;
   int rc = plan_build(ctx, pl, db, n, ids, req_query);
@@ -2625,13 +2704,25 @@ int hhg_viterbi_search_batch(hhg_ctx* ctx, const hhg_db* db, int n, const int32_
   pl->nm_mode = -1;
   if (db->raw) {
     // every query needs its own null model: factor it in while the plan's operand stream is built
-    if (columnscore < 0 || columnscore > 3) return fail(HHG_EINVAL, "hhg_viterbi_search_batch: columnscore %d", columnscore);
-    if (!ctx->has_q_pav) return fail(HHG_EINVAL, "hhg_viterbi_search_batch: raw shard needs q_pav in hhg_query_set_batch");
-    if (columnscore == 0 && !pb) return fail(HHG_EINVAL, "hhg_viterbi_search_batch: columnscore 0 needs pb");
     memset(ctx->h_pb, 0, sizeof ctx->h_pb);
     if (pb) memcpy(ctx->h_pb, pb, sizeof ctx->h_pb);
     CK(ctx->d_pb.ensure(20));
     CK(cudaMemcpyAsync(ctx->d_pb.p, ctx->h_pb, sizeof ctx->h_pb, cudaMemcpyHostToDevice, ctx->stream));
+    if (columnscore == 5) {
+      // query-independent: divide the cols of the distinct targets the requests name (not the whole shard); the
+      // operand stream and k_backtrace then read cols unfused.  The shard is left unprepared (hhg.h).
+      std::vector<int> uniq(ids, ids + n);
+      std::sort(uniq.begin(), uniq.end());
+      uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
+      std::vector<LocalBgSeg> segs;
+      segs.reserve(uniq.size());
+      for (int t : uniq) segs.push_back(LocalBgSeg{db->col_off[t], db->col_off[t], db->L[t], 0});
+      hhg_db* wdb = const_cast<hhg_db*>(db);
+      wdb->prepared = false;
+      wdb->cols_version++;
+      rc = local_bg_launch(ctx, segs, db->cols_raw.p, db->cols.p, ctx->h_pb);
+      if (rc != HHG_OK) return rc;
+    }
     CK(cudaStreamSynchronize(ctx->stream));
     pl->nm_mode = columnscore;
   }
@@ -2952,9 +3043,10 @@ static int mac_realign_impl(hhg_ctx* ctx, const hhg_db* db, bool batch, int n, c
   if (!fuse && !db->prepared) return fail(HHG_EINVAL, "%s: shard has no null model applied", who);
   if (fuse) {
     // every query needs its own null model (columnscore / pb as in hhg_viterbi_search_batch)
-    if (columnscore < 0 || columnscore > 3) return fail(HHG_EINVAL, "%s: columnscore %d", who, columnscore);
-    if (!ctx->mac_has_q_pav) return fail(HHG_EINVAL, "%s: raw shard needs q_pav in hhg_mac_query_set_batch", who);
-    if (columnscore == 0 && !pb) return fail(HHG_EINVAL, "%s: columnscore 0 needs pb", who);
+    if (columnscore < 0 || columnscore == 4 || columnscore > 5) return fail(HHG_EINVAL, "%s: columnscore %d", who, columnscore);
+    if (columnscore != 5 && !ctx->mac_has_q_pav)
+      return fail(HHG_EINVAL, "%s: raw shard needs q_pav in hhg_mac_query_set_batch", who);
+    if ((columnscore == 0 || columnscore == 5) && !pb) return fail(HHG_EINVAL, "%s: columnscore %d needs pb", who, columnscore);
   }
   if (excl_off && (!excl_i || !excl_j)) return fail(HHG_EINVAL, "%s: excl_off without excl_i/excl_j", who);
   CK(cudaSetDevice(ctx->device));
@@ -3062,11 +3154,11 @@ static int mac_realign_impl(hhg_ctx* ctx, const hhg_db* db, bool batch, int n, c
   CK(ctx->mac_map.ensure((size_t)n));
   CK(cudaMemcpyAsync(ctx->mac_i64.p, h64.data(), h64.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(ctx->mac_i32.p, h32.data(), h32.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+  float h_pb_mac[20] = {};
   if (fuse) {
-    float h_pb[20] = {};
-    if (pb) memcpy(h_pb, pb, sizeof h_pb);
+    if (pb) memcpy(h_pb_mac, pb, sizeof h_pb_mac);
     CK(ctx->mac_pb.ensure(20));
-    CK(cudaMemcpyAsync(ctx->mac_pb.p, h_pb, sizeof h_pb, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->mac_pb.p, h_pb_mac, sizeof h_pb_mac, cudaMemcpyHostToDevice, ctx->stream));
   }
   const long long* d64 = ctx->mac_i64.p;
   const long long *d_rec0 = d64, *d_tr_off = d64 + n, *d_cell_off = d64 + 2 * n, *d_row_off = d64 + 3 * n,
@@ -3144,7 +3236,13 @@ static int mac_realign_impl(hhg_ctx* ctx, const hhg_db* db, bool batch, int n, c
     const int last = w0 + m - 1;
     const long long ncell = cell_off[last] + (long long)(Lqr[last] + 1) * (Lt[last] + 1);
     CK(cudaMemsetAsync(ctx->mac_bt.p, 0, (size_t)ncell, ctx->stream));
-    if (fuse) {
+    if (fuse && columnscore == 5) {
+      // the template's raw records, locally corrected, into the request's copy (query-independent)
+      std::vector<LocalBgSeg> segs(m);
+      for (int r = 0; r < m; ++r) segs[r] = LocalBgSeg{db->col_off[target[w0 + r]], rec0[w0 + r], Lt[w0 + r], 0};
+      const int rc = local_bg_launch(ctx, segs, db->cols_raw.p, ctx->mac_cols.p, h_pb_mac);
+      if (rc != HHG_OK) return rc;
+    } else if (fuse) {
       for (int r0 = 0; r0 < m; r0 += 65535) {
         const int k = std::min(m - r0, 65535);
         k_mac_gather_cols<<<dim3(4, k), 128, 0, ctx->stream>>>(

@@ -61,7 +61,8 @@ def realign_batch(ctx: capi.Context, db: capi.TargetDB, queries, hits, q_pav=Non
                   shift=-0.03, mact=0.35):
     """realign for every query of a batch at once.  queries: list of (q_p, q_tr) as realign takes them; hits[q]: the
     Viterbi hits of query q (e.g. runner.BatchViterbiRunner.alignment); q_pav [nq, 20], columnscore and pb: the null
-    model of a raw shard (hhg_mac_realign_batch).  Round k realigns the k-th hit (in irep order) of every (query, target)
+    model of a raw shard (hhg_mac_realign_batch; with 5 pass the queries' p divided by capi.query_local_background).
+    Round k realigns the k-th hit (in irep order) of every (query, target)
     pair of all queries in one call, excluding the MAC alignments found for that pair before.  Returns one
     {(target, irep): MacResult} per query."""
     capi.mac_query_set_batch(ctx, [(q[0], capi.log2lin(q[1])) for q in queries], q_pav)

@@ -14,6 +14,8 @@ def search(ctx: capi.Context, db: capi.TargetDB, csdb: capi.CsDB, q_p, q_tr, q_p
            altali=4, smin=20.0, cs_names=None, db_names=None, **pf_kwargs):
     """q_p/q_tr: prepared query (Viterbi); q_prefilter_p: HMM::p of the prefilter-pseudocount copy of the query
     (q_tmp, src/hhblits.cpp:1149-1163; defaults to q_p).  Returns (survivor ids in the TARGET shard, list of runner.Hit).
+    Under column score 5 (db prepared by apply_null_model(pb=pb, columnscore=5)) pass q_p divided by
+    capi.query_local_background and the undivided p as q_prefilter_p: the prefilter never sees the division.
 
     The prefilter's survivors are entries of the cs219 index; the reference carries them to the Viterbi stage BY NAME
     (src/hhprefilter.cpp:561-590, then a lookup in the hhm/a3m index), because the two indices of a real database
@@ -57,9 +59,13 @@ def search_staged(ctx: capi.Context, db: capi.StagedDB, csdb: capi.CsDB, q_p, q_
     hhg_db_stage call), the query's null model is applied to the staged records (columnscore / pb as in
     TargetDB.apply_null_model) and the same runner aligns them.  Returns what search() returns over a resident raw shard
     of the whole database after apply_null_model(q_pav, pb, columnscore): survivor ids and Hit.target are GLOBAL ids.
-    The survivors of one query must fit db (HhgError otherwise, with the sizes needed)."""
+    The survivors of one query must fit db (HhgError otherwise, with the sizes needed).  With columnscore 5, q_p is the
+    undivided query: the prefilter profile is built from it and the Viterbi stage aligns its local composition
+    correction (capi.query_local_background with the context's half window), as hhblits does."""
     prof = capi.build_prefilter_profile(q_p if q_prefilter_p is None else q_prefilter_p, q_pav, lib219,
                                         pf_kwargs.get("score_offset", 50), pf_kwargs.get("bit_factor", 4))
+    if columnscore == 5:
+        q_p = capi.query_local_background(ctx, q_p, pb)
     ids = _to_targets(prefilter.prefilter_db(csdb, prof, **pf_kwargs), db.store, csdb, cs_names, db_names)
     if not len(ids):
         return ids, []
@@ -77,10 +83,12 @@ def search_batch_staged(ctx: capi.Context, db: capi.StagedDB, csdb: capi.CsDB, q
     in one call, then the batch runner aligns every query with its own survivors, the null model of each query fused
     into the search (so q_pav of every query is used: pass (q_p, q_tr, q_pav[, q_prefilter_p]) as for search_batch).
     Returns what search_batch() returns over a resident raw shard of the whole database, with GLOBAL ids.  The union
-    must fit db."""
+    must fit db.  With columnscore 5 each q_p is undivided, as in search_staged."""
     so, bf = pf_kwargs.get("score_offset", 50), pf_kwargs.get("bit_factor", 4)
     profs = [capi.build_prefilter_profile(q[0] if len(q) < 4 or q[3] is None else q[3], q[2], lib219, so, bf)
              for q in queries]
+    if columnscore == 5:
+        queries = [(capi.query_local_background(ctx, q[0], pb),) + tuple(q[1:]) for q in queries]
     ids = [_to_targets(x, db.store, csdb, cs_names, db_names)
            for x in prefilter.prefilter_db_batch(csdb, profs, **pf_kwargs)]
     rq = np.concatenate([np.full(len(x), q, np.int32) for q, x in enumerate(ids)])

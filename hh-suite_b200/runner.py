@@ -125,7 +125,8 @@ class BatchViterbiRunner:
     src/hhblits_omp.cpp:119-160): pass 0 aligns every request, pass k > 0 realigns the (query, target) requests whose
     previous hit scored above smin with all earlier paths of that pair masked -- one hhg_viterbi_search_batch call per
     pass for all queries.  The queries are those of the last capi.query_set_batch; over a raw shard the null model is
-    applied per query (columnscore / pb as in capi.viterbi_search_batch).  No early stopping and no per-batch ss
+    applied per query (columnscore / pb as in capi.viterbi_search_batch; with 5 the queries of the batch must be divided
+    by capi.query_local_background, and the shard is left unprepared).  No early stopping and no per-batch ss
     consensus: split the requests by hhg_set_use_ss beforehand if the ss term is wanted for some of them."""
 
     def __init__(self, ctx: capi.Context, db: capi.TargetDB, altali: int = 4, smin: float = 20.0, columnscore: int = 1,

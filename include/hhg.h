@@ -103,11 +103,29 @@ int hhg_db_create(hhg_ctx* ctx, int n, const int32_t* L, const int64_t* p_off, c
  * (what AddAminoAcidPseudocounts leaves in HMM::p, src/hhfunc.cpp:176-178) and pav[n*20] holds each
  * target's average amino-acid frequencies (HMM::pav).  The query-dependent step of PrepareTemplateHMM
  * -- HMM::IncludeNullModelInHMM, src/hhhmm.cpp:2059 -- then runs on the GPU for every new query:
- * hhg_db_apply_null_model(columnscore = par.columnscore: 0 pb, 1 (q.pav+t.pav)/2, 2 t.pav, 3 q.pav). */
+ * hhg_db_apply_null_model(columnscore = par.columnscore: 0 pb, 1 (q.pav+t.pav)/2, 2 t.pav, 3 q.pav, 5 the local
+ * amino-acid composition correction below).  Column score 4 and anything else are refused with HHG_EINVAL.
+ *
+ * Column score 5 (-sc 5 / -scwin D of hhblits, hhsearch and hhalign): HMM::DivideBySqrtOfLocalBackgroundFreqs
+ * (src/hhhmm.cpp:1979-2035), case 5 of IncludeNullModelInHMM.  Every column i = 1..L of a profile is divided by
+ * sqrt(fac * pnul[i]), pnul[i][a] = 10*pb[a] + the sum of p[.][a] over the 2D+1 columns around i (the whole profile
+ * when L <= 2D+1), computed in the reference's float order, so the results are bit-identical.  It reads pb[20], needs
+ * no q_pav and does not depend on the query, so a shard prepared with it serves every query.  The QUERY is divided too
+ * (PrepareQueryHMM, src/hhfunc.cpp:157-159): run hhg_query_local_background on its p before hhg_query_set /
+ * hhg_mac_query_set(_batch) / hhg_query_set_batch, and build the prefilter profile from the undivided p, as hhblits does
+ * (src/hhblits.cpp:1127-1163).  D is the context's half window (hhg_set_scwin, default 40). */
 int hhg_db_create_raw(hhg_ctx* ctx, int n, const int32_t* L, const int64_t* p_off, const int64_t* tr_off,
                       const int64_t* ss_off, const float* p, const float* tr, const uint8_t* ss,
                       const float* pav, hhg_db** out);
 int hhg_db_apply_null_model(hhg_ctx* ctx, hhg_db* db, const float* q_pav, const float* pb, int columnscore);
+/* The half window D of column score 5 (par.half_window_size_local_aa_bg_freqs, -scwin; the CLIs clamp it to >= 1) for
+ * every following call of this context that applies column score 5.  Default 40; D < 1 is HHG_EINVAL. */
+int hhg_set_scwin(hhg_ctx* ctx, int half_window);
+/* Column score 5 for a query: p[(L+2)*20] (host, HMM::p after CalculateAminoAcidBackground) is divided in place, rows
+ * 1..L, with the context's D and the background pb[20]; rows 0 and L+1 are left as they are, like the reference leaves
+ * them.  Runs the shard's kernel on one profile (upload, launch, download, synchronise).  L outside [1, 32767] is
+ * HHG_EINVAL. */
+int hhg_query_local_background(hhg_ctx* ctx, int L, const float* pb, float* p);
 
 /* ---- database load straight from HHM text records (SURVEY 8a rows a10 + a11; 8f-1) ------------------------
  * Replaces, once per database instead of once per (query, target):
@@ -422,6 +440,11 @@ int hhg_viterbi_search(hhg_ctx* ctx, const hhg_db* db, int n, const int32_t* ids
  *                         (hhg_db_create_raw / _hhm / _packed): the query-dependent null model
  *                         (HMM::IncludeNullModelInHMM, columnscore / pb as in hhg_db_apply_null_model) is applied per
  *                         query while the plan's operand stream is built -- no per-query pass over the whole shard.
+ *                         columnscore 5 (query-independent, pb required, q_pav not needed) instead divides the prepared
+ *                         emissions of the distinct targets the requests name, in the shard itself, with the context's
+ *                         half window: the call leaves the shard UNPREPARED, and a following hhg_viterbi_search or
+ *                         hhg_mac_realign on it is refused until hhg_db_apply_null_model.  The queries must have been
+ *                         divided by hhg_query_local_background.  A prepared shard ignores columnscore / pb.
  *                         excl_*: as in hhg_viterbi_search, per request (the alternative alignments of
  *                         ViterbiRunner::alignment for every query of the batch in one call); steps are checked against
  *                         that request's query length and target length.  NULL = no path exclusions. */
@@ -576,8 +599,9 @@ int hhg_mac_realign(hhg_ctx* ctx, const hhg_db* db, int n, const int32_t* target
  *   shard is raw (may be NULL otherwise).  hhg_mac_query_set == a batch of one without q_pav.
  * hhg_mac_realign_batch, request r: query req_query[r] against target[r]; every other argument as in hhg_mac_realign,
  *   path_cap >= sum(Lq of the request's query + Lt + 2).  Raw shard (hhg_db_create_raw / _hhm / _packed): the null
- *   model of the request's query (HMM::IncludeNullModelInHMM, columnscore / pb as in hhg_viterbi_search_batch) is
- *   applied to a copy of the template's raw records, so the result does not depend on hhg_db_apply_null_model; a
+ *   model of the request's query (HMM::IncludeNullModelInHMM, columnscore / pb as in hhg_viterbi_search_batch; column
+ *   score 5 with the context's half window) is applied to a copy of the template's raw records, so the result does not
+ *   depend on hhg_db_apply_null_model and the shard is not changed; a
  *   prepared shard is read as it is and columnscore / pb are ignored.  The requests are cut, in order, into memory waves
  *   whose scratch (about 6 bytes per cell) stays within the context's backtrace budget (HHG_MAX_BT_GB); the results
  *   do not depend on the cut.  Results are bit-identical to hhg_db_apply_null_model + hhg_mac_query_set +
